@@ -3,7 +3,7 @@ PY ?= python
 
 .PHONY: build test test-gpu bench smoke sass-check reference clean
 
-build:            ## nvcc -gencode arch=compute_100a,code=sm_100a -> swiftllm_b200/libswiftllm_b200.so
+build:            ## nvcc -gencode arch=compute_90a,code=sm_90a -> swiftllm_b200/libswiftllm_b200.so
 	$(PY) -m swiftllm_b200.build
 
 test: build       ## CPU suite: oracle vs golden vectors, host logic, C-ABI surface, gloo TP, dry runs, mirrors

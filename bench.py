@@ -5,8 +5,9 @@
   python bench.py --impl reference ...                            # CPU arm: torch-eager oracle port on host cores
   torchrun --nproc-per-node N bench.py --gpus N ...               # N > 1: tensor parallel (heads / FFN columns)
 
-Workload (BASELINE.json configs[1]): Llama-3-8B shapes, bf16, pure decode, batch 256, every sequence at
+Workload (BASELINE.json configs[1]): Llama-3-8B shapes, bf16, pure decode, batch 64, every sequence at
 seq_len 4096, block_size 16, synthetic seeded weights N(0, 0.02) and a KV cache pre-filled with N(0, 1).
+Batch 64 x 4096 tokens is a 32 GiB KV cache: with the 16 GB of weights it fits one 80 GB H100.
 A "step" is one LlamaModel.forward over the batch = one new token per sequence.
 
 One JSON line on stdout (rank 0).  Keys beyond the base contract:
@@ -15,6 +16,10 @@ One JSON line on stdout (rank 0).  Keys beyond the base contract:
              of the metadata and one D2H read of the sampled tokens inside the timed region
   roofline   paged-decode kernel: algorithmic bytes / mean CUDA-event duration of its launches over K eager steps
   cpu_baseline  the oracle (CPU torch-eager restatement of the reference forward) on a bounded sample
+
+--dump-outputs DIR writes, after the timed steps, the token ids the last timed step of each path returned
+(DIR/tokens.npy for the device-resident path, DIR/e2e_tokens.npy for the public-API path) as float64.  Weights, KV
+cache and prompts are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -51,7 +56,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", type=str, default="ours", choices=["ours", "reference"])
-    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--seqlen", type=int, default=4096)
     ap.add_argument("--model", type=str, default="llama3-8b", choices=["llama3-8b", "llama3-70b", "tiny"])
     ap.add_argument("--layers", type=int, default=0, help="override the layer count (debug only; marks the run reduced)")
@@ -86,6 +91,8 @@ def parse():
     ap.add_argument("--no-live-traffic", action="store_true", help="skip the ncu DRAM-byte measurement of the decode kernel")
     ap.add_argument("--no-prefill", action="store_true")
     ap.add_argument("--cpu-sample-seqs", type=int, default=8)
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the token ids of the last timed step as DIR/<name>.npy (float64)")
     ap.add_argument("--profile-range", type=int, default=0,
                     help="profiling aid: run this many eager decode steps inside cudaProfilerStart/Stop and exit "
                          "(use with ncu --profile-from-start off); prints no bench line")
@@ -220,23 +227,18 @@ def workload_config(args, cfg, n):
     return {"workload": f"{args.model} pure decode, batch {args.batch}, seq_len {args.seqlen}, block_size 16 "
                         f"(BASELINE.json configs[1])",
             "layers": cfg["num_hidden_layers"], "global_batch": args.batch, "seq_len": args.seqlen,
-            "parallelism": f"tp{n}", "l2": "inputs larger than L2 (KV working set and weights >> 126 MB)"}
+            "parallelism": f"tp{n}", "l2": "inputs larger than L2 (KV working set and weights >> 50 MB)"}
 
 
 
-# --------------------------------------------------------------------------- reference Triton arm (north_star: "next to the
-# reference's own Triton path on one B200"): the UNMODIFIED reference under baseline/_ref/src, in its own process
+# --------------------------------------------------------------------------- reference Triton arm: the UNMODIFIED reference
+# under baseline/_ref/src, in its own process
 def run_reference_triton(args, dtypes):
-    """Runs scripts/ref_triton_bench.py once per dtype BEFORE this process allocates its own 143 GB (both need most of the
+    """Runs scripts/ref_triton_bench.py once per dtype BEFORE this process allocates its own KV cache (both need most of the
     GPU).  Same workload, same public call (LlamaModel.forward: host lists in, host ints out), same step count and
     warm-up, CUDA events around the K steps.  Returns {dtype: json-line-or-error}."""
     out = {}
     script = os.path.join(ROOT, "scripts", "ref_triton_bench.py")
-    last = {}
-    try:
-        last = json.load(open(os.path.join(ROOT, "profiles", "ref_triton_last_measured.json")))
-    except Exception:  # noqa: BLE001
-        pass
     for dt in dtypes:
         stage(f"reference Triton arm ({dt}) ...")
         env = dict(os.environ, REF_DTYPE=dt, REF_BATCH=str(args.batch), REF_SEQLEN=str(args.seqlen),
@@ -258,8 +260,6 @@ def run_reference_triton(args, dtypes):
                           f"128-way unrolled kernel)"}
         except Exception as e:  # noqa: BLE001
             d = {"error": str(e)[:300]}
-        if "error" in d and dt in last:
-            d["last_measured"] = last[dt]            # committed record of an earlier run on a B200 (profiles/), labelled as such
         d["wall_s"] = round(time.perf_counter() - t0, 1)
         out[dt] = d
     return out
@@ -535,9 +535,12 @@ def run_ours(args):
     # ---- e2e: public API, host lists in, host ints out
     state = {"ids": ids0}
 
+    last_e2e = {}
+
     def step_e2e():
         toks = model.forward(state["ids"], sids, lens)            # H2D metadata + D2H tokens inside
         state["ids"] = [[t] for t in toks]
+        last_e2e["toks"] = toks
 
     for _ in range(max(args.warmup, 3)):
         step_e2e()
@@ -568,13 +571,18 @@ def run_ours(args):
         if graph is not None:
             graph["meta"][:B].copy_(graph["tokens"].to(torch.int32))     # next step's ids = sampled tokens, on device
             graph["graph"].replay()
+            state["resident"] = graph["tokens"]
         else:
-            model.forward_async(state["ids"], sids, lens)
+            state["resident"] = model.forward_async(state["ids"], sids, lens)
 
     for _ in range(max(args.warmup, 3)):
         step_resident()
     ms_val = timed(step_resident, args.steps)
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "tokens.npy"), torch.as_tensor(state["resident"]).to(torch.float64).cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "e2e_tokens.npy"), np.asarray(last_e2e["toks"], dtype=np.float64))
 
     stage("roofline pass (events around every decode-attention launch)")
     # ---- roofline of the dominant kernel (paged decode attention): eager steps with events around each launch
@@ -597,17 +605,13 @@ def run_ours(args):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     else:
-        peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not a measured peak)"
     achieved = alg_bytes / (pa_ms * 1e-3) / 1e9
     traffic, traffic_src = None, None
     if rank == 0 and not args.no_live_traffic:
         stage("live DRAM traffic of the decode kernel (ncu subprocess)")
         torch.cuda.synchronize()
         traffic, traffic_src = measure_traffic_live(args, mc, n)
-    tpath = os.path.join(ROOT, "profiles", "paged_attn_traffic.json")
-    if traffic is None and os.path.exists(tpath) and n == 1 and args.model == "llama3-8b" and B == 256 and S == 4096 and not args.layers:
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj["dram_bytes_read"] + tj["dram_bytes_write"], f"committed constant, {tj['source']} (live ncu: {traffic_src})"
 
     # rank 0 may have spent ~10 s in the ncu subprocess: meet at a HOST-level barrier (NCCL, no watchdog) before the next
     # collective step, so that no rank sits inside a fused exchange kernel (which traps after ~1-2 minutes of spinning) meanwhile
@@ -621,7 +625,7 @@ def run_ours(args):
                               full_getter=synthetic_getter(seed=0, std=0.02, device=dev))
     pa_gen = os.environ.get("SLLM_PAGED_ATTN_GEN", "")
     kname = "paged_attn_kernel (gen 1: cp.async + mma.sync)" if pa_gen == "1" else \
-        "paged_attn_tc_kernel (gen 2: tcgen05 + TMA, persistent)"
+        "paged_attn_tc_kernel (gen 2: TMA + wgmma, persistent)"
 
     # ---- optional: prefill tokens/s (secondary metric of BASELINE.json)
     prefill = None
@@ -638,8 +642,8 @@ def run_ours(args):
                 model.free_seqs_resources(psids)
             for _ in range(2):
                 step_prefill()
-            ms_p = timed(step_prefill, 3)
-            prefill = {"value": Bp * Lp / (ms_p / 3 * 1e-3), "unit": UNIT, "batch": Bp, "prompt_len": Lp}
+            ms_p = timed(step_prefill, args.steps)
+            prefill = {"value": Bp * Lp / (ms_p / args.steps * 1e-3), "unit": UNIT, "batch": Bp, "prompt_len": Lp}
         except Exception as e:  # noqa: BLE001
             prefill = {"error": str(e)[:200]}
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Data-plane-only generation with swiftllm_b200.LlamaModel - the counterpart of the reference's examples/offline.py (same
 worker API and call order: load_weights -> profile_num_blocks -> init_kvcache_and_swap -> forward for the prompts -> forward
-per generated token).  Needs a B200 (there is no CPU path).
+per generated token).  Needs an H100 (there is no CPU path).
 
     python examples/offline.py --model-path /data/Llama-3-8B            # real checkpoint + its HF tokenizer
     python examples/offline.py --synthetic llama3-8b                     # seeded random weights, random token ids

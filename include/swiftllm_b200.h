@@ -1,5 +1,5 @@
 /*
- * swiftllm_b200.h - C ABI of the B200-native (sm_100a) data plane that replaces every kernel in
+ * swiftllm_b200.h - C ABI of the H100-native (sm_90a) data plane that replaces every kernel in
  * swiftLLM's `swiftllm/worker/kernels/` plus the native `swiftllm_c` module.
  *
  * Drop-in boundary: the reference binds its kernels as Python functions on torch tensors (one wrapper
@@ -14,7 +14,7 @@
  *   - all functions enqueue on `stream` (a cudaStream_t) and return immediately;
  *   - return value: 0 on success, non-zero on error (`sllm_last_error()` gives the message).  Invalid
  *     shapes are rejected before anything is launched (the reference raises AssertionError there);
- *   - no CPU fallback exists: on a non-sm_100 device every launch fails with an error.
+ *   - no CPU fallback exists: on a non-sm_90 device every launch fails with an error.
  *
  * Reference paths below are relative to the swiftLLM repository root.
  */

@@ -304,6 +304,27 @@ def gen_model(swiftllm):
     save("model_tiny", **arrays)
 
 
+def gen_model_config():
+    """The reference's LlamaModelConfig over GQA / MHA / scaled-RoPE / legacy-key configs: every attribute it defines and its
+    KV-slot size per dtype (tests/golden/model_config.json; read by tests/test_host_logic.py)."""
+    import importlib.util
+    from swiftllm_b200.model_config import LLAMA3_8B
+    spec = importlib.util.spec_from_file_location("ref_model_config", os.path.join(ref_shim.REFERENCE_ROOT, "swiftllm", "model_config.py"))
+    ref = importlib.util.module_from_spec(spec); spec.loader.exec_module(ref)
+    base = dict(LLAMA3_8B)
+    cfgs = [base, dict(base, rope_scaling={"factor": 8.0, "low_freq_factor": 1.0}),
+            {k: v for k, v in base.items() if k not in ("num_key_value_heads", "rope_theta", "rope_scaling")},
+            dict({k: v for k, v in base.items() if k != "rope_theta"}, rotary_base=12345), dict(base, rope_scaling=2.0)]
+    cases = []
+    for c in cfgs:
+        theirs = ref.LlamaModelConfig(c)
+        cases.append({"config": c, "attrs": vars(theirs),
+                      "kvslot_size": {"float16": theirs.get_kvslot_size(torch.float16), "bfloat16": theirs.get_kvslot_size(torch.bfloat16)}})
+    with open(os.path.join(GOLDEN, "model_config.json"), "w") as f:
+        json.dump({"reference": "interestingLSY/swiftLLM swiftllm/model_config.py", "cases": cases}, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 def main():
     os.makedirs(GOLDEN, exist_ok=True)
     swiftllm = ref_shim.import_reference()
@@ -312,6 +333,7 @@ def main():
     gen_prefill(swiftllm)
     gen_block_mgmt(swiftllm)
     gen_model(swiftllm)
+    gen_model_config()
 
 
 if __name__ == "__main__":

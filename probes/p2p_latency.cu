@@ -4,8 +4,8 @@
 //   2. peer read bandwidth: one kernel on GPU0 sums a buffer that lives on GPU1 with 16-byte volatile loads (the one-shot path)
 //      for sizes from 256 KiB (a decode exchange at TP 8: 32 rows x 8 KiB) to 128 MiB (a prefill exchange);
 //   3. peer write bandwidth: 16-byte stores into GPU1's memory (the two-shot path's all-gather half).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -o probes/build/p2p_latency probes/p2p_latency.cu
-// Run on a box with >= 2 GPUs: gpurun --gpus 2 -- 'probes/build/p2p_latency'
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -o probes/build/p2p_latency probes/p2p_latency.cu
+// Run on a machine with >= 2 GPUs: probes/build/p2p_latency
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

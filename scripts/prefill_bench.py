@@ -28,7 +28,7 @@ def run(gen, Bp, L, nq=32, nkv=8, D=128, iters=10):
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / iters
     flops = 4 * nq * D * Bp * L * (L + 1) / 2
-    return {"gen": "gen1-mma.sync" if gen == "1" else "gen2-tcgen05", "Bp": Bp, "L": L, "ms": ms, "tflops": flops / (ms * 1e-3) / 1e12}, o
+    return {"gen": "gen1-mma.sync" if gen == "1" else "gen2-wgmma", "Bp": Bp, "L": L, "ms": ms, "tflops": flops / (ms * 1e-3) / 1e12}, o
 
 def run_fa2(Bp, L, nq=32, nkv=8, D=128, iters=10):
     """flash_attn_varlen_func exactly as the reference calls it (causal, same cu_seqlens for q and k)."""

@@ -1,5 +1,5 @@
-"""A few launches of the tcgen05 prefill attention kernel at 8 x 4096 tokens (Llama-3-8B heads, bf16) for an ncu capture:
-    ncu --set full --import-source on -k regex:prefill_attn_tc_kernel --launch-skip 2 --launch-count 1 -o gpurun_out/prefill_tc python scripts/prefill_one.py"""
+"""A few launches of the wgmma prefill attention kernel at 8 x 4096 tokens (Llama-3-8B heads, bf16) for an ncu capture:
+    ncu --set full --import-source on -k regex:prefill_attn_tc_kernel --launch-skip 2 --launch-count 1 -o profile_out/prefill_tc python scripts/prefill_one.py"""
 import os, sys, types
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import torch

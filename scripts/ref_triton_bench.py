@@ -31,10 +31,9 @@ if DTYPE == "bf16":
                     npatched += t.count(".float16"); open(p, "w").write(t2)
     assert npatched >= 10, npatched
 # Triton JIT cache.  The reference's phase-1 kernel unrolls seq_block_size / block_size = 128 pages (tl.static_range,
-# paged_attn.py:88) and is specialised three times on cur_layer: ~8 minutes of ptxas on a cold cache.  A cache built once on a
-# B200 box of this image (scripts/gpu_r2_session_e.sh) is kept under baseline/_ref/triton_cache/<dtype> (git-ignored,
-# travels with the repo snapshot): the UNMODIFIED kernels, compiled by the same Triton, only not recompiled.
-# REF_TRITON_CACHE_DIR overrides the location (the warm-up script points it at gpurun_out/).
+# paged_attn.py:88) and is specialised three times on cur_layer: ~8 minutes of ptxas on a cold cache.  A cache built
+# once may be kept under baseline/_ref/triton_cache/<dtype> (git-ignored): the UNMODIFIED kernels, compiled by the same
+# Triton, only not recompiled.  REF_TRITON_CACHE_DIR overrides the location.
 cache = os.environ.get("REF_TRITON_CACHE_DIR") or os.path.join(ROOT, "baseline", "_ref", "triton_cache", DTYPE)
 packed = os.path.join(ROOT, "baseline", "_ref", f"triton_cache_{DTYPE}.tar.gz")     # how the cache travels (it compresses 8x)
 if not os.environ.get("REF_TRITON_CACHE_DIR") and not os.path.isdir(cache) and os.path.exists(packed):

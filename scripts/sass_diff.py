@@ -4,7 +4,7 @@
     python scripts/sass_diff.py save  <dir>      # dump one normalised .sass per kernel into <dir>
     python scripts/sass_diff.py check <dir>      # report kernels whose instruction stream changed / appeared / vanished
     python scripts/sass_diff.py manifest <json> "<where validated>"   # hash of every kernel's normalised SASS: written after the
-                                                 # whole `pytest -m gpu` suite, smoke() and bench.py passed on a B200 with this
+                                                 # whole `pytest -m gpu` suite, smoke() and bench.py passed on an H100 with this
                                                  # exact build (tests/test_cabi.py holds later builds to it)
 
 Used when a validated kernel's SOURCE is refactored without a GPU at hand (e.g. moved into a shared template): an

@@ -82,8 +82,8 @@ def main():
     rows = {ev.key: [ev.count, float(ev.device_time_total)] for ev in prof.key_averages()
             if ev.device_type == DeviceType.CUDA and ev.device_time_total > 0}
     tot = sum(r[1] for r in rows.values())
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    path = os.path.join(ROOT, "gpurun_out", f"shard_launches_tp{args.tp}_b{B}_s{S}{args.tag}.csv")
+    os.makedirs(os.path.join(ROOT, "profile_out"), exist_ok=True)
+    path = os.path.join(ROOT, "profile_out", f"shard_launches_tp{args.tp}_b{B}_s{S}{args.tag}.csv")
     with open(path, "w") as f:
         f.write("kernel,launches_per_step,us_per_step,us_per_launch,share\n")
         for k, (c, us) in sorted(rows.items(), key=lambda kv: -kv[1][1]):

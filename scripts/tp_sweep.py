@@ -8,7 +8,7 @@ For every variant (exchange kernel x lm_head sharding x rotary/store fusion) it 
 warms up, and times K CUDA-graph replays of the decode step (device-resident token feedback, barrier + synchronize on both
 sides, max over ranks) and K steps through the public API (host lists in / ints out).  One JSON line per variant on stdout
 (rank 0).  `--profile NAME` additionally records a per-kernel launch list of that variant on rank 0 with the torch profiler
-(CUPTI; ncu cannot be used on a multi-rank command) and writes it to gpurun_out/tp_sweep_launches_n<N>_<NAME>.csv.
+(CUPTI; ncu cannot be used on a multi-rank command) and writes it to profile_out/tp_sweep_launches_n<N>_<NAME>.csv.
 This is a development tool: the contract numbers come from bench.py."""
 import argparse
 import gc
@@ -69,7 +69,7 @@ def main():
     gen = torch.Generator().manual_seed(7)
     ids0 = [[int(t)] for t in torch.randint(0, mc.vocab_size, (B,), generator=gen)]
     sids, lens = list(range(B)), [S] * B
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
+    os.makedirs(os.path.join(ROOT, "profile_out"), exist_ok=True)
 
     def barrier():
         dist.barrier(); torch.cuda.synchronize()
@@ -137,7 +137,7 @@ def main():
                             if ev.device_type == DeviceType.CUDA and ev.device_time_total > 0:
                                 rows[ev.key] = [ev.count, float(ev.device_time_total)]
                         tot = sum(r[1] for r in rows.values())
-                        path = os.path.join(ROOT, "gpurun_out", f"tp_sweep_launches_n{n}_{name.replace('+', '_')}_b{B}.csv")
+                        path = os.path.join(ROOT, "profile_out", f"tp_sweep_launches_n{n}_{name.replace('+', '_')}_b{B}.csv")
                         with open(path, "w") as f:
                             f.write("kernel,launches_per_step,us_per_step,share\n")
                             for k, (c, us) in sorted(rows.items(), key=lambda kv: -kv[1][1]):

@@ -1,4 +1,4 @@
-"""swiftllm_b200 - B200-native (sm_100a) data plane for swiftLLM's `LlamaModel`.
+"""swiftllm_b200 - H100-native (sm_90a) data plane for swiftLLM's `LlamaModel`.
 
 Mirrors the reference package surface that belongs to the hot path:
     swiftllm_b200.EngineConfig, swiftllm_b200.LlamaModel           (swiftllm/__init__.py:2,9)

@@ -1,6 +1,6 @@
 """ctypes binding of libswiftllm_b200.so (the C ABI declared in include/swiftllm_b200.h).
 
-There is NO fallback: if the library is missing or the device is not sm_100 every kernel wrapper raises.
+There is NO fallback: if the library is missing or the device is not sm_90 every kernel wrapper raises.
 """
 from __future__ import annotations
 
@@ -58,7 +58,7 @@ def lib() -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise NativeLibraryError(
-                f"{LIB_PATH} not found: build it with `python -m swiftllm_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} not found: build it with `python -m swiftllm_b200.build` (nvcc, sm_90a). "
                 "swiftllm_b200 has no CPU or PyTorch fallback path.")
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
@@ -123,7 +123,7 @@ _checked_devices = set()
 
 
 def require_device(t: torch.Tensor):
-    """Fail loudly if a tensor is not on an sm_100 GPU."""
+    """Fail loudly if a tensor is not on an sm_90 (H100) GPU."""
     if not t.is_cuda:
         raise RuntimeError("swiftllm_b200 kernels need CUDA tensors (no CPU path exists)")
     idx = t.device.index if t.device.index is not None else torch.cuda.current_device()

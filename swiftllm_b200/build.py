@@ -1,8 +1,8 @@
-"""Builds the sm_100a data-plane library IN-TREE: swiftllm_b200/libswiftllm_b200.so (plain nvcc, C ABI).
+"""Builds the sm_90a data-plane library IN-TREE: swiftllm_b200/libswiftllm_b200.so (plain nvcc, C ABI).
 
     python -m swiftllm_b200.build            # incremental (per-file objects under swiftllm_b200/csrc/build/)
 
-The .so is git-ignored but travels to the GPU box with the snapshot.  sm_100a only: no other -gencode.
+The .so and the objects are build products (git-ignored).  sm_90a only: no other -gencode.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ _VARIANT = os.environ.get("SLLM_BUILD_VARIANT", "")
 OBJ = os.path.join(CSRC, "build" + ("_" + _VARIANT if _VARIANT else ""))
 LIB = os.path.join(HERE, "libswiftllm_b200" + ("_" + _VARIANT if _VARIANT else "") + ".so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"] + os.environ.get("SLLM_NVCC_EXTRA", "").split()
 
 

@@ -1,7 +1,6 @@
 // Tensor-parallel exchange, low-latency variant (SURVEY.md §8 f-3): reduce-scatter + residual add + RMSNorm + all-gather in
-// ONE kernel with NO barrier.  Measured on B200/NVSwitch (profiles/r2_p2p_latency_n2.log): a flag round trip costs 5.5 us,
-// i.e. every "publish a flag, wait for everybody's flag" barrier costs ~3 us one way, and the flag-based two-shot kernel
-// (allreduce_norm.cu) pays two of them plus a peer-load round trip plus a system fence: ~28 us per exchange for 2 MiB.
+// ONE kernel with NO barrier.  Every "publish a flag, wait for everybody's flag" barrier costs one NVLink round trip, and the
+// flag-based two-shot kernel (allreduce_norm.cu) pays two of them plus a peer-load round trip plus a system fence.
 // Here data is PUSHED and carries its own validity (the NCCL "LL" idea): every 8-byte unit that crosses NVLink is
 // {4 bytes of payload, 4-byte epoch tag}; a receiver polls the data itself until the tag equals the epoch of this exchange.
 // One one-way latency per phase, nothing else:
@@ -226,7 +225,7 @@ extern "C" int sllm_allreduce_add_rmsnorm_ll(const void* partial, void* const* h
     if (sm_count[dev] == 0) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sm_count[dev] = n > 0 ? n : 148;
+        sm_count[dev] = n > 0 ? n : 132;
     }
     const int64_t cap = 2LL * sm_count[dev];                         // every CTA must be resident: 2 x 512 threads per SM always fit
     const unsigned grid = (unsigned)(num_tokens < cap ? num_tokens : cap);

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a data-plane kernels.
+// Shared helpers for the sm_90a data-plane kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -61,7 +61,7 @@ template <typename T> __device__ __forceinline__ Vec8<T> ld_vec8_stream(const T*
     return *reinterpret_cast<Vec8<T>*>(&u);
 }
 
-// shared-memory address of a generic pointer (operand of cp.async / ldmatrix / mbarrier / TMA / UMMA descriptors)
+// shared-memory address of a generic pointer (operand of cp.async / ldmatrix / mbarrier / TMA / wgmma descriptors)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -59,8 +59,8 @@ int sllm_device_check(int device) {
         sllm::set_error("cudaGetDeviceProperties(%d): %s", device, cudaGetErrorString(e));
         return (int)e;
     }
-    if (p.major != 10) {
-        sllm::set_error("device %d is sm_%d%d; this library contains sm_100a code only (no fallback path)",
+    if (p.major != 9) {
+        sllm::set_error("device %d is sm_%d%d; this library contains sm_90a code only (no fallback path)",
                         device, p.major, p.minor);
         return 1;
     }

@@ -1,5 +1,5 @@
 // Warp-level tensor-core and async-copy primitives (cp.async / ldmatrix / mma.sync m16n8k16) used by the
-// first-generation attention kernels.  The tcgen05/TMA kernels live in *_tc.cu and do not use these.
+// first-generation attention kernels.  The TMA/wgmma kernels live in *_tc.cu and do not use these.
 #pragma once
 #include "common.cuh"
 

@@ -253,7 +253,7 @@ static int num_sms() {                       // of the CURRENT device (a process
     if (sms[dev] == 0) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms[dev] = n > 0 ? n : 148;
+        sms[dev] = n > 0 ? n : 132;
     }
     return sms[dev];
 }
@@ -279,7 +279,7 @@ int launch_paged_tc(const void* q, const void* k_cache, const void* v_cache, con
                     int split_tokens, int num_splits, int cur_layer, int num_layers, int nq, int nkv, int max_blocks_per_seq,
                     int64_t num_blocks, int64_t q_row_stride, sllm_dtype_t dtype, int num_sms, cudaStream_t stream);
 
-// SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements, debugging); default: tcgen05/TMA
+// SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements, debugging); default: TMA/wgmma
 // whenever the shape is covered (head_dim 128, block_size 16).
 static int forced_generation() {
     const char* e = getenv("SLLM_PAGED_ATTN_GEN");      // re-read every call so tests can toggle it
@@ -368,7 +368,7 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
         }
         return 0;
     }
-    SLLM_REQUIRE(forced_generation() != 2, "paged_attention: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the tcgen05 kernel");
+    SLLM_REQUIRE(forced_generation() != 2, "paged_attention: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
     if (head_dim == 128) { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 128>(p, num_decoding_seqs, max_seq_len, st))); }
     else { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 64>(p, num_decoding_seqs, max_seq_len, st))); }
     return 0;

@@ -1,22 +1,18 @@
-// Paged (decode) attention, generation 2: persistent, warp-specialised tcgen05 + TMA kernel (sm_100a).
+// Paged (decode) attention, generation 2: persistent, warp-specialised TMA + wgmma kernel (sm_90a).
 //
 // Reference being replaced: swiftllm/worker/kernels/paged_attn.py:9-108 (+ :111-149 via the merge kernel of
 // paged_attn.cu when a sequence is split).  Shapes served: head_dim 128, block_size 16, GQA group <= 16, fp16/bf16.
 //
 // One persistent CTA per SM walks a static list of work items (sequence, kv head, split).  Per 128-token tile:
-//   warp 0 (1 lane)  TMA producer: reads 8 block-table entries, issues one 4-D tensor-map load per 16-token page
-//                    for K and one for V (4 KiB each, SWIZZLE_128B atoms [token-group][d-half][8 tok][64 d]) into a
-//                    3-stage ring, completion on mbarriers; Q of the item is a 2-box TMA load.
-//   warp 1 (1 lane)  MMA issuer:  S^T[128 tok x 16 heads] = K_tile (A, K-major) . Q^T (B, K-major)         (8 UMMAs)
-//                                 O^T[128 d  x 16 heads] = V_tile^T (A, MN-major) . P^T (B, K-major)        (8 UMMAs)
-//                    accumulators in TMEM (2 x 16 columns each, double buffered), completion via tcgen05.commit.
-//   warps 2-5        softmax: thread = token row of S^T (tcgen05.ld), scale + tail mask, tile max across the 128
-//                    threads, p = exp2(s - m) -> bf16/fp16 P^T tile in shared memory (B operand of the PV UMMA);
-//                    the same threads then own one d-row of O^T and fold each tile's O into fp32 registers with the
-//                    running-max correction (no TMEM read-modify-write), and write o / the split partial.
-// Tokens are the MMA M dimension (the transposed problem), so no tensor work is spent on padded query rows and the
-// softmax uses all 128 threads; the GQA group is the N dimension (padded to 16 by reading neighbouring heads whose
-// columns are simply never read back).
+//   warp 4 (K) / warp 5 (V)  TMA producers: read 8 block-table entries, issue one 4-D tensor-map load per 16-token page
+//                    (4 KiB, SWIZZLE_128B atoms [token-group][d-half][8 tok][64 d]) into 3-stage rings, completion on
+//                    mbarriers; warp 4 also loads Q of the item (a 2-box TMA load).
+//   warps 0-3        one warpgroup that issues the MMAs and runs the softmax, accumulators in registers:
+//                    S^T[128 tok x NP heads] = K_tile (A, K-major) . Q^T (B, K-major)       (2 x 8 wgmma m64nNPk16)
+//                    tile max per head across the warpgroup, p = exp2(s - m) -> bf16/fp16 P^T tile in shared memory,
+//                    O^T[128 d x NP heads] = alpha * O^T + V_tile^T (A, MN-major) . P^T (B, K-major)   (2 x 8 wgmma)
+// Tokens are the MMA M dimension (the transposed problem), so no tensor work is spent on padded query rows; the GQA
+// group is the N dimension (padded to NP = 8 or 16 by reading neighbouring heads whose columns are never written back).
 // HBM roofline: algorithmic bytes = sum_i len_i * nkv * 128 * 2 * sizeof(T) + 2 * Bd * nq * 128 * sizeof(T).
 #include <mutex>
 #include <unordered_map>
@@ -32,13 +28,12 @@ constexpr int TC_BS = 16;                 // tokens per page
 constexpr int TC_TILE = 128;              // tokens per pipeline stage (8 pages)
 constexpr int TC_KSTAGES = 3;             // K ring (freed as soon as S = K.Q^T of the tile has completed)
 constexpr int TC_VSTAGES = 3;             // V ring (freed when O = V^T.P^T of the tile has completed)
-constexpr int TC_THREADS = 224;           // warp 0: K+Q producer, warp 1: MMA issuer, warps 2..5: softmax, warp 6: V producer
-constexpr int TC_NPAD = 16;               // UMMA N (heads, padded)
+constexpr int TC_THREADS = 192;           // warps 0..3: MMA + softmax warpgroup, warp 4: K+Q producer, warp 5: V producer
+constexpr int TC_NPAD = 16;               // largest wgmma N (heads, padded)
 constexpr int TC_K_BYTES = TC_TILE * TC_D * 2;                 // 32 KiB per K (or V) tile
 constexpr int TC_Q_BYTES = 2 * TC_NPAD * 128;                  // [half][16 rows][128 B] = 4 KiB
 constexpr int TC_P_BYTES = 2 * TC_NPAD * 128;                  // [token half][16 rows][128 B] = 4 KiB
-constexpr int TC_SMEM_BYTES = (TC_KSTAGES + TC_VSTAGES) * TC_K_BYTES + 2 * TC_Q_BYTES + 2 * TC_P_BYTES + 2048;
-constexpr int TC_TMEM_COLS = 64;          // S: 2 x 16, O: 2 x 16
+constexpr int TC_SMEM_BYTES = (TC_KSTAGES + TC_VSTAGES) * TC_K_BYTES + 2 * TC_Q_BYTES + TC_P_BYTES + 2048;
 
 struct TcParams {
     const int32_t* block_table; const int32_t* seq_ids; const int32_t* seq_lens;
@@ -53,9 +48,6 @@ struct Barriers {       // all mbarriers of the CTA (shared memory)
     uint64_t k_full[TC_KSTAGES], k_empty[TC_KSTAGES];
     uint64_t v_full[TC_VSTAGES], v_empty[TC_VSTAGES];
     uint64_t q_full[2], q_empty[2];
-    uint64_t s_full[2], s_empty[2];
-    uint64_t p_full[2];
-    uint64_t o_full[2], o_empty[2];
 };
 
 struct Item { int seq, kvh, split, split_start, split_len, ntiles; };
@@ -73,27 +65,6 @@ __device__ __forceinline__ bool get_item(const TcParams& p, int idx, Item& it) {
     it.ntiles = (it.split_len + TC_TILE - 1) / TC_TILE;
     return true;
 }
-
-// Walks this CTA's work items tile by tile (every role runs the same deterministic schedule).
-struct TileCursor {
-    int idx;            // global item index (blockIdx.x + k * gridDim.x)
-    Item it;
-    int j;              // tile within the item
-    uint32_t t, n;      // tile / item counters of this CTA
-    bool valid;
-    __device__ __forceinline__ void seek(const TcParams& p) {            // position on the next non-empty item
-        valid = false;
-        while (idx < p.num_items) {
-            if (get_item(p, idx, it)) { valid = true; j = 0; return; }
-            idx += gridDim.x;
-        }
-    }
-    __device__ __forceinline__ void init(const TcParams& p) { idx = blockIdx.x; t = 0; n = 0; seek(p); }
-    __device__ __forceinline__ void advance(const TcParams& p) {
-        t++;
-        if (++j == it.ntiles) { n++; idx += gridDim.x; seek(p); }
-    }
-};
 
 // One producer warp streams either the K or the V tiles (plus Q when IS_K): 32 block-table entries are fetched per
 // 4 tiles (prefetched one group ahead), lanes 0..7 each issue the TMA of one page.
@@ -151,20 +122,21 @@ __device__ __forceinline__ void producer_loop(const TcParams& p, const CUtensorM
     }
 }
 
-template <typename T, int G>      // G = number of S/O columns read back (GQA group padded to 4, 8 or 16)
+template <typename T, int NP>      // NP = wgmma N: the GQA group padded to 8 or 16
 __global__ void __launch_bounds__(TC_THREADS, 1) paged_attn_tc_kernel(const __grid_constant__ CUtensorMap kmap,
                                                                       const __grid_constant__ CUtensorMap vmap,
                                                                       const __grid_constant__ CUtensorMap qmap,
                                                                       const TcParams p) {
+    constexpr int NR = NP / 2;                 // accumulator registers per m64 block
+    constexpr int NH = NP / 4;                 // head columns owned by one thread
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* k_sm = smem;                                            // [KSTAGES][32 KiB]
     uint8_t* v_sm = smem + TC_KSTAGES * TC_K_BYTES;                  // [VSTAGES][32 KiB]
     uint8_t* q_sm = v_sm + TC_VSTAGES * TC_K_BYTES;                  // [2][4 KiB]
-    uint8_t* p_sm = q_sm + 2 * TC_Q_BYTES;                           // [2][4 KiB]
-    uint8_t* misc = p_sm + 2 * TC_P_BYTES;                           // barriers, tmem base, reduction scratch
+    uint8_t* p_sm = q_sm + 2 * TC_Q_BYTES;                           // [4 KiB]
+    uint8_t* misc = p_sm + TC_P_BYTES;                               // barriers, reduction scratch
     Barriers* bars = reinterpret_cast<Barriers*>(misc);
-    uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(misc + 256);
-    float* red = reinterpret_cast<float*>(misc + 320);               // [2 parity][4 warps][16] + [4][16] sums
+    float* red = reinterpret_cast<float*>(misc + 256);               // [2 parity][4 warps][16] maxima, [4 warps][16] sums
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = p.nq / p.nkv;
@@ -175,213 +147,182 @@ __global__ void __launch_bounds__(TC_THREADS, 1) paged_attn_tc_kernel(const __gr
         for (int i = tid; i < (TC_KSTAGES + TC_VSTAGES) * TC_K_BYTES / 16; i += TC_THREADS) z[i] = make_uint4(0, 0, 0, 0);
     }
     if (tid == 0) {
-        for (int i = 0; i < TC_KSTAGES; i++) { mbar_init(smem_u32(&bars->k_full[i]), 1); mbar_init(smem_u32(&bars->k_empty[i]), 1); }
-        for (int i = 0; i < TC_VSTAGES; i++) { mbar_init(smem_u32(&bars->v_full[i]), 1); mbar_init(smem_u32(&bars->v_empty[i]), 1); }
-        for (int i = 0; i < 2; i++) {
-            mbar_init(smem_u32(&bars->q_full[i]), 1); mbar_init(smem_u32(&bars->q_empty[i]), 1);
-            mbar_init(smem_u32(&bars->s_full[i]), 1); mbar_init(smem_u32(&bars->s_empty[i]), 128);
-            mbar_init(smem_u32(&bars->p_full[i]), 128);
-            mbar_init(smem_u32(&bars->o_full[i]), 1); mbar_init(smem_u32(&bars->o_empty[i]), 128);
-        }
+        for (int i = 0; i < TC_KSTAGES; i++) { mbar_init(smem_u32(&bars->k_full[i]), 1); mbar_init(smem_u32(&bars->k_empty[i]), 128); }
+        for (int i = 0; i < TC_VSTAGES; i++) { mbar_init(smem_u32(&bars->v_full[i]), 1); mbar_init(smem_u32(&bars->v_empty[i]), 128); }
+        for (int i = 0; i < 2; i++) { mbar_init(smem_u32(&bars->q_full[i]), 1); mbar_init(smem_u32(&bars->q_empty[i]), 128); }
         mbar_fence_init();
         tma_prefetch_desc(&kmap); tma_prefetch_desc(&vmap); tma_prefetch_desc(&qmap);
     }
-    if (warp == 1) tmem_alloc<TC_TMEM_COLS>(smem_u32(tmem_base_s));
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_base_s;
 
-    if (warp == 0) {
+    if (warp == 4) {
         producer_loop<true>(p, &kmap, &qmap, k_sm, bars->k_full, bars->k_empty, TC_KSTAGES, bars, q_sm, g, lane);
-    } else if (warp == 6) {
+    } else if (warp == 5) {
         producer_loop<false>(p, &vmap, &qmap, v_sm, bars->v_full, bars->v_empty, TC_VSTAGES, bars, q_sm, g, lane);
-    } else if (warp == 1) {
-        // =========================================================== MMA issuer: two in-order queues, polled.  The whole warp
-        // runs the loop converged (votes keep the control flow provably uniform) and one elected lane issues, so ptxas keeps
-        // the UMMA descriptors in uniform registers instead of wrapping every UTCHMMA in a uniformisation loop.
-        {
-            constexpr uint32_t IDESC_S = make_instr_desc(128, TC_NPAD, UmmaFmt<T>::value, 0, 0);   // A K-major, B K-major
-            constexpr uint32_t IDESC_O = make_instr_desc(128, TC_NPAD, UmmaFmt<T>::value, 1, 0);   // A MN-major (V^T)
-            constexpr uint32_t FULL = 0xffffffffu;
-            const uint32_t tm = __shfl_sync(FULL, tmem, 0);
-            const uint64_t dk0 = make_smem_desc(smem_u32(k_sm), 16, p.k_sbo);
-            const uint64_t dq0 = make_smem_desc(smem_u32(q_sm), 16, 1024);
-            const uint64_t dv0 = make_smem_desc(smem_u32(v_sm), p.v_lbo, p.v_sbo);
-            const uint64_t dp0 = make_smem_desc(smem_u32(p_sm), 16, 1024);
-            TileCursor cs, cp;                  // next S tile / next PV tile
-            cs.init(p); cp.init(p);
-            uint32_t spins = 0;
-            while (cp.valid) {
-                bool progressed = false;
-                if (cs.valid) {
-                    const uint32_t t = cs.t;
-                    const int stage = t % TC_KSTAGES, b = t & 1, qb = cs.n & 1;
-                    const bool ready = (cs.j > 0 || mbar_test_wait(smem_u32(&bars->q_full[qb]), (cs.n >> 1) & 1)) &&
-                                       mbar_test_wait(smem_u32(&bars->k_full[stage]), (t / TC_KSTAGES) & 1) &&
-                                       mbar_test_wait(smem_u32(&bars->s_empty[b]), ((t >> 1) & 1) ^ 1);
-                    if (__all_sync(FULL, ready)) {
-                        tc_fence_after();
-                        const bool last = cs.j == cs.it.ntiles - 1;
-                        if (elect_one()) {
-                            const uint64_t kd = dk0 + (uint64_t)((stage * TC_K_BYTES) >> 4);
-                            const uint64_t qd = dq0 + (uint64_t)((qb * TC_Q_BYTES) >> 4);
-#pragma unroll
-                            for (int ks = 0; ks < 8; ks++)      // 16 d per UMMA; d-half = ks / 4
-                                umma_ss(tm + b * 16, kd + (uint64_t)(((ks >> 2) * p.half_stride + (ks & 3) * 32) >> 4),
-                                        qd + (uint64_t)(((ks >> 2) * 2048 + (ks & 3) * 32) >> 4), IDESC_S, ks > 0);
-                            umma_commit(smem_u32(&bars->s_full[b]));
-                            umma_commit(smem_u32(&bars->k_empty[stage]));                       // K tile consumed
-                            if (last) umma_commit(smem_u32(&bars->q_empty[qb]));                // Q buffer reusable
-                        }
-                        __syncwarp();
-                        cs.advance(p);
-                        progressed = true;
-                    }
-                }
-                if (cp.t < cs.t || !cs.valid) {
-                    const uint32_t t = cp.t;
-                    const int stage = t % TC_VSTAGES, b = t & 1;
-                    const bool ready = mbar_test_wait(smem_u32(&bars->p_full[b]), (t >> 1) & 1) &&
-                                       mbar_test_wait(smem_u32(&bars->v_full[stage]), (t / TC_VSTAGES) & 1) &&
-                                       mbar_test_wait(smem_u32(&bars->o_empty[b]), ((t >> 1) & 1) ^ 1);
-                    if (__all_sync(FULL, ready)) {
-                        tc_fence_after();
-                        if (elect_one()) {
-                            const uint64_t vd = dv0 + (uint64_t)((stage * TC_K_BYTES) >> 4);
-                            const uint64_t pd = dp0 + (uint64_t)((b * TC_P_BYTES) >> 4);
-#pragma unroll
-                            for (int kt = 0; kt < 8; kt++)      // 16 tokens (one page) per UMMA
-                                umma_ss(tm + 32 + b * 16, vd + (uint64_t)((kt * p.page_stride) >> 4),
-                                        pd + (uint64_t)(((kt >> 2) * 2048 + (kt & 3) * 32) >> 4), IDESC_O, kt > 0);
-                            umma_commit(smem_u32(&bars->o_full[b]));
-                            umma_commit(smem_u32(&bars->v_empty[stage]));
-                        }
-                        __syncwarp();
-                        cp.advance(p);
-                        progressed = true;
-                    }
-                }
-                if (progressed) spins = 0;
-                else if (++spins > (1u << 24)) {
-                    if (lane == 0) printf("sllm: MMA issuer watchdog (block %d, S tile %u, PV tile %u)\n", blockIdx.x, cs.t, cp.t);
-                    __trap();
-                }
-            }
-        }
     } else {
-        // =========================================================== softmax / accumulate warps (128 threads)
-        const int quad = warp & 3;                     // TMEM lane quadrant this warp may access
-        const int row = quad * 32 + lane;              // token row of S^T, d row of O^T
-        const uint32_t tlane = (uint32_t)(quad * 32) << 16;
-        const int sw = warp - 2;                       // 0..3 index for the reduction scratch
-        uint32_t t = 0;
+        // =========================================================== MMA + softmax warpgroup (warps 0..3)
+        // Thread (warp w, lane l) owns token rows / d rows r = 16 w + l / 4 + 8 hi + 64 mb (hi, mb in {0, 1}) and the head
+        // columns hc(c) = 2 (l % 4) + (c & 1) + 8 (c >> 1), c < NH, of the S^T and O^T tiles.
+        const uint64_t dk0 = make_smem_desc(smem_u32(k_sm), 16, p.k_sbo);
+        const uint64_t dq0 = make_smem_desc(smem_u32(q_sm), 16, 1024);
+        const uint64_t dv0 = make_smem_desc(smem_u32(v_sm), p.v_lbo, p.v_sbo);
+        const uint64_t dp0 = make_smem_desc(smem_u32(p_sm), 16, 1024);
+        const int r0 = 16 * warp + (lane >> 2);
+        int hc[NH];
+#pragma unroll
+        for (int c = 0; c < NH; c++) hc[c] = 2 * (lane & 3) + (c & 1) + 8 * (c >> 1);
+        uint32_t t = 0, n = 0;
         T* const out = reinterpret_cast<T*>(p.o);
         for (int idx = blockIdx.x; idx < p.num_items; idx += gridDim.x) {
             Item it;
             if (!get_item(p, idx, it)) continue;
-            float m_run[G], l_part[G], acc[G], alpha_prev[G];
+            const int qb = n & 1;
+            mbar_wait(smem_u32(&bars->q_full[qb]), (n >> 1) & 1);
+            float m_run[NH], l_part[NH];
+            float acc[2][NR];
 #pragma unroll
-            for (int h = 0; h < G; h++) { m_run[h] = -INFINITY; l_part[h] = 0.f; acc[h] = 0.f; alpha_prev[h] = 0.f; }
-
-            auto fold_o = [&](uint32_t tt) {            // acc = acc * alpha(tt) + O_tile(tt)
-                const int b = tt & 1;
-                mbar_wait(smem_u32(&bars->o_full[b]), (tt >> 1) & 1);
-                tc_fence_after();
-                uint32_t r[G];
-                tmem_ld<G>(tmem + tlane + 32 + b * 16, r);
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(smem_u32(&bars->o_empty[b]));
+            for (int c = 0; c < NH; c++) { m_run[c] = -INFINITY; l_part[c] = 0.f; }
 #pragma unroll
-                for (int h = 0; h < G; h++) acc[h] = acc[h] * alpha_prev[h] + __uint_as_float(r[h]);
-            };
+            for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                for (int e = 0; e < NR; e++) acc[mb][e] = 0.f;
 
             for (int j = 0; j < it.ntiles; j++, t++) {
-                const int b = t & 1;
-                mbar_wait(smem_u32(&bars->s_full[b]), (t >> 1) & 1);
-                tc_fence_after();
-                uint32_t r[G];
-                tmem_ld<G>(tmem + tlane + b * 16, r);
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(smem_u32(&bars->s_empty[b]));
-
-                const bool valid = j * TC_TILE + row < it.split_len;
-                float x[G], wmax[G];
+                // ---- S^T = K . Q^T
+                const int ks_ = t % TC_KSTAGES;
+                mbar_wait(smem_u32(&bars->k_full[ks_]), (t / TC_KSTAGES) & 1);
+                float s[2][NR];
+                {
+                    const uint64_t kd = dk0 + (uint64_t)((ks_ * TC_K_BYTES) >> 4);
+                    const uint64_t qd = dq0 + (uint64_t)((qb * TC_Q_BYTES) >> 4);
+                    wgmma_fence();
 #pragma unroll
-                for (int h = 0; h < G; h++) {
-                    x[h] = valid ? __uint_as_float(r[h]) * p.scale_log2e : -INFINITY;
-                    wmax[h] = warp_max(x[h]);
+                    for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                        for (int kk = 0; kk < 8; kk++) {     // 16 d per wgmma; d-half = kk / 4
+                            const uint64_t a = kd + (uint64_t)((mb * 8 * p.k_sbo + (kk >> 2) * p.half_stride + (kk & 3) * 32) >> 4);
+                            const uint64_t b = qd + (uint64_t)(((kk >> 2) * 2048 + (kk & 3) * 32) >> 4);
+                            if constexpr (NP == 8) wgmma_m64n8k16_ss<T, 0, 0>(s[mb], a, b, kk > 0);
+                            else wgmma_m64n16k16_ss<T, 0, 0>(s[mb], a, b, kk > 0);
+                        }
+                    wgmma_commit();
+                    wgmma_wait<0>();
                 }
-                float* rp = red + (t & 1) * 64;
-                if (lane == 0) {
+                mbar_arrive(smem_u32(&bars->k_empty[ks_]));                            // K tile consumed
+                if (j == it.ntiles - 1) mbar_arrive(smem_u32(&bars->q_empty[qb]));     // Q buffer reusable
+
+                // ---- scale + tail mask, tile max per head across the 128 token rows
+                float mx[NH];
 #pragma unroll
-                    for (int h = 0; h < G; h++) rp[sw * 16 + h] = wmax[h];
+                for (int c = 0; c < NH; c++) mx[c] = -INFINITY;
+#pragma unroll
+                for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                    for (int e = 0; e < NR; e++) {
+                        const int tok = j * TC_TILE + mb * 64 + r0 + 8 * ((e >> 1) & 1);
+                        const int c = (e & 1) + 2 * (e >> 2);
+                        s[mb][e] = tok < it.split_len ? s[mb][e] * p.scale_log2e : -INFINITY;
+                        mx[c] = fmaxf(mx[c], s[mb][e]);
+                    }
+                float* rp = red + (t & 1) * 64;
+#pragma unroll
+                for (int c = 0; c < NH; c++) {
+#pragma unroll
+                    for (int o = 4; o < 32; o <<= 1) mx[c] = fmaxf(mx[c], __shfl_xor_sync(0xffffffffu, mx[c], o));
+                    if (lane < 4) rp[warp * 16 + hc[c]] = mx[c];
                 }
                 named_bar_sync(1, 128);
-                float pj[G];
+                float alpha[NH];
 #pragma unroll
-                for (int h = 0; h < G; h++) {
+                for (int c = 0; c < NH; c++) {
+                    const int h = hc[c];
                     const float mt = fmaxf(fmaxf(rp[h], rp[16 + h]), fmaxf(rp[32 + h], rp[48 + h]));
-                    const float mn = fmaxf(m_run[h], mt);                  // finite: every tile has a valid token
-                    const float a = fast_exp2_tc(m_run[h] - mn);
-                    pj[h] = fast_exp2_tc(x[h] - mn);
-                    l_part[h] = l_part[h] * a + pj[h];
-                    m_run[h] = mn;
-                    x[h] = a;                                              // x[] now carries alpha(j) = exp2(m(j-1) - m(j))
+                    const float mn = fmaxf(m_run[c], mt);                  // finite: every tile has a valid token
+                    alpha[c] = fast_exp2_tc(m_run[c] - mn);
+                    l_part[c] *= alpha[c];
+                    m_run[c] = mn;
                 }
-                // P^T tile (B operand of the PV UMMA): [token half][16 head rows][128 B], SWIZZLE_128B.
-                // Buffer b was last read by PV(t-2), whose completion (o_full) these threads observed last iteration.
-                {
-                    uint8_t* pb = p_sm + b * TC_P_BYTES + (row >> 6) * 2048 + (row & 7) * 2;
-                    const int c = (row & 63) >> 3;
+                // p = exp2(s - m) -> P^T tile (B operand of the PV wgmma): [token half][16 head rows][128 B], SWIZZLE_128B.
+                // The previous PV wgmma that read the buffer completed (wgmma_wait) before any thread got here.
 #pragma unroll
-                    for (int h = 0; h < G; h++)
-                        *reinterpret_cast<T*>(pb + h * 128 + ((c ^ (h & 7)) << 4)) = Traits<T>::from_f(pj[h]);
-                }
+                for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                    for (int e = 0; e < NR; e++) {
+                        const int row = mb * 64 + r0 + 8 * ((e >> 1) & 1);
+                        const int c = (e & 1) + 2 * (e >> 2);
+                        const float pv = fast_exp2_tc(s[mb][e] - m_run[c]);
+                        l_part[c] += pv;
+                        const int h = hc[c];
+                        *reinterpret_cast<T*>(p_sm + mb * 2048 + h * 128 + ((((row & 63) >> 3) ^ (h & 7)) << 4) + (row & 7) * 2) =
+                            Traits<T>::from_f(pv);
+                    }
                 fence_proxy_async();
-                mbar_arrive(smem_u32(&bars->p_full[b]));
-                if (j > 0) fold_o(t - 1);
-#pragma unroll
-                for (int h = 0; h < G; h++) alpha_prev[h] = x[h];
-            }
-            fold_o(t - 1);
+                named_bar_sync(1, 128);
 
-            // ---- finalise the item: l = sum over the 128 token-threads, out[h][d=row] = acc / l
-            float* rp = red + 128;                                         // [4 warps][16] scratch for the sums
-            float lsum[G];
+                // ---- O^T = alpha * O^T + V^T . P^T
 #pragma unroll
-            for (int h = 0; h < G; h++) lsum[h] = warp_sum(l_part[h]);
-            // (every thread passed >= 1 per-tile barrier since the previous item's reads of rp)
-            if (lane == 0) {
+                for (int mb = 0; mb < 2; mb++)
 #pragma unroll
-                for (int h = 0; h < G; h++) rp[sw * 16 + h] = lsum[h];
+                    for (int e = 0; e < NR; e++) acc[mb][e] *= alpha[(e & 1) + 2 * (e >> 2)];
+                const int vs = t % TC_VSTAGES;
+                mbar_wait(smem_u32(&bars->v_full[vs]), (t / TC_VSTAGES) & 1);
+                {
+                    const uint64_t vd = dv0 + (uint64_t)((vs * TC_K_BYTES) >> 4);
+                    wgmma_fence();
+#pragma unroll
+                    for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                        for (int kt = 0; kt < 8; kt++) {     // 16 tokens (one page) per wgmma
+                            const uint64_t a = vd + (uint64_t)((mb * p.half_stride + kt * p.page_stride) >> 4);
+                            const uint64_t b = dp0 + (uint64_t)(((kt >> 2) * 2048 + (kt & 3) * 32) >> 4);
+                            if constexpr (NP == 8) wgmma_m64n8k16_ss<T, 1, 0>(acc[mb], a, b, 1);
+                            else wgmma_m64n16k16_ss<T, 1, 0>(acc[mb], a, b, 1);
+                        }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                }
+                mbar_arrive(smem_u32(&bars->v_empty[vs]));
+            }
+            n++;
+
+            // ---- finalise the item: l = sum over the 128 token rows, out[h][d] = acc / l
+            float* rp = red + 128;
+#pragma unroll
+            for (int c = 0; c < NH; c++) {
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) l_part[c] += __shfl_xor_sync(0xffffffffu, l_part[c], o);
+                if (lane < 4) rp[warp * 16 + hc[c]] = l_part[c];
             }
             named_bar_sync(1, 128);
+            float L[NH];
 #pragma unroll
-            for (int h = 0; h < G; h++) {
-                if (h < g) {
-                    const float L = (rp[h] + rp[16 + h]) + (rp[32 + h] + rp[48 + h]);
-                    const float val = acc[h] / L;
-                    const int head = it.kvh * g + h;
-                    if (p.num_splits == 1) {
-                        out[((int64_t)it.seq * p.nq + head) * TC_D + row] = Traits<T>::from_f(val);
-                    } else {
-                        const int64_t pi = ((int64_t)it.seq * p.nq + head) * p.num_splits + it.split;
-                        p.part_o[pi * TC_D + row] = val;
-                        if (row == 0) p.part_lse[pi] = log2f(L) + m_run[h];
+            for (int c = 0; c < NH; c++) {
+                const int h = hc[c];
+                L[c] = (rp[h] + rp[16 + h]) + (rp[32 + h] + rp[48 + h]);
+            }
+            named_bar_sync(1, 128);          // rp is rewritten by the next item
+#pragma unroll
+            for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+                for (int e = 0; e < NR; e++) {
+                    const int c = (e & 1) + 2 * (e >> 2);
+                    const int h = hc[c];
+                    if (h < g) {
+                        const int d = mb * 64 + r0 + 8 * ((e >> 1) & 1);
+                        const float val = acc[mb][e] / L[c];
+                        const int head = it.kvh * g + h;
+                        if (p.num_splits == 1) {
+                            out[((int64_t)it.seq * p.nq + head) * TC_D + d] = Traits<T>::from_f(val);
+                        } else {
+                            const int64_t pi = ((int64_t)it.seq * p.nq + head) * p.num_splits + it.split;
+                            p.part_o[pi * TC_D + d] = val;
+                            if (d == 0) p.part_lse[pi] = log2f(L[c]) + m_run[c];
+                        }
                     }
                 }
-            }
         }
     }
-
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<TC_TMEM_COLS>(tmem);
 }
 
 }  // namespace sllm
@@ -499,12 +440,12 @@ int launch_paged_tc(const void* q, const void* k_cache, const void* v_cache, con
         paged_attn_tc_kernel<TT, GG><<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(kmap, vmap, qmap, p);                  \
     } while (0)
     if (dtype == SLLM_F16) {
-        if (g <= 4) SLLM_TC_LAUNCH(__half, 4); else if (g <= 8) SLLM_TC_LAUNCH(__half, 8); else SLLM_TC_LAUNCH(__half, 16);
+        if (g <= 8) SLLM_TC_LAUNCH(__half, 8); else SLLM_TC_LAUNCH(__half, 16);
     } else {
-        if (g <= 4) SLLM_TC_LAUNCH(__nv_bfloat16, 4); else if (g <= 8) SLLM_TC_LAUNCH(__nv_bfloat16, 8); else SLLM_TC_LAUNCH(__nv_bfloat16, 16);
+        if (g <= 8) SLLM_TC_LAUNCH(__nv_bfloat16, 8); else SLLM_TC_LAUNCH(__nv_bfloat16, 16);
     }
 #undef SLLM_TC_LAUNCH
-    return check_launch("paged_attention(tcgen05)");
+    return check_launch("paged_attention(wgmma)");
 }
 
 }  // namespace sllm

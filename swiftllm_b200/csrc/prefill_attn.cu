@@ -53,13 +53,13 @@ extern "C" int sllm_prefill_attention(const void* q, const void* k, const void* 
     SLLM_REQUIRE(q_row_stride >= (int64_t)nq * head_dim && k_row_stride >= (int64_t)nkv * head_dim && v_row_stride >= (int64_t)nkv * head_dim &&
                  q_row_stride % 8 == 0 && k_row_stride % 8 == 0 && v_row_stride % 8 == 0, "prefill_attention: bad row strides");
     cudaStream_t st = (cudaStream_t)stream;
-    // SLLM_PREFILL_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements); default: tcgen05/TMA for head_dim 128
+    // SLLM_PREFILL_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements); default: TMA/wgmma for head_dim 128
     const char* gen_env = getenv("SLLM_PREFILL_ATTN_GEN");
     const int gen = (gen_env && gen_env[0] == '1') ? 1 : (gen_env && gen_env[0] == '2') ? 2 : 0;
     if (gen != 1 && dtype <= SLLM_BF16 && tc_prefill_supported(head_dim, num_prefill_tokens))
         return launch_prefill_tc(q, k, v, o, start_locs, seq_lens, softmax_scale * 1.4426950408889634f, num_prefill_seqs,
                                  max_prefill_len, num_prefill_tokens, nq, nkv, q_row_stride, k_row_stride, v_row_stride, dtype, st);
-    SLLM_REQUIRE(gen != 2, "prefill_attention: SLLM_PREFILL_ATTN_GEN=2 but the shape is not covered by the tcgen05 kernel");
+    SLLM_REQUIRE(gen != 2, "prefill_attention: SLLM_PREFILL_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
     if (head_dim == 128) { SLLM_DISPATCH_DTYPE(dtype, return (launch_prefill<T, 128>(q, k, v, o, start_locs, seq_lens, softmax_scale, num_prefill_seqs, max_prefill_len, nq, nkv, q_row_stride, k_row_stride, v_row_stride, st))); }
     else { SLLM_DISPATCH_DTYPE(dtype, return (launch_prefill<T, 64>(q, k, v, o, start_locs, seq_lens, softmax_scale, num_prefill_seqs, max_prefill_len, nq, nkv, q_row_stride, k_row_stride, v_row_stride, st))); }
     return 0;

@@ -4,7 +4,7 @@
 // batch), which is what SARATHI-style piggybacking (BASELINE.json configs[2]) needs.  Definition = the one that makes
 // a prompt processed in chunks equal to the same prompt processed at once (oracle/kernels.py:
 // prefix_prefill_attention_exact).  Both generations of the prefill kernel are instantiated with PAGED = true:
-//   gen 2 (prefill_attn_tc_kernel.cuh): tcgen05 + TMA page gather, head_dim 128, block_size 16
+//   gen 2 (prefill_attn_tc_kernel.cuh): TMA page gather + wgmma, head_dim 128, block_size 16
 //   gen 1 (prefill_attn_kernel.cuh):    cp.async page gather + mma.sync, head_dim 64 / 128, any block_size
 // Roofline: tensor-bound; FLOPs = 4 * nq * D * sum_i (prefix_i * L_i + L_i (L_i + 1) / 2).
 #include <stdlib.h>
@@ -46,7 +46,7 @@ static int launch_prefill_paged_tc(const void* q, const void* k_cache, const voi
                  "prefill_attention_paged: cuTensorMapEncodeTiled failed");
     PtParams p;
     p.o = o; p.start_locs = start_locs; p.seq_lens = chunk_lens; p.scale_log2e = scale_log2e; p.nq = nq; p.nkv = nkv;
-    dim3 grid((max_chunk_len + 2 * PT_BQ - 1) / (2 * PT_BQ), nq, num_seqs);
+    dim3 grid((max_chunk_len + PT_BQ - 1) / PT_BQ, nq, num_seqs);
     if (dtype == SLLM_F16) {
         static unsigned long long c = 0;
         if (first_use_on_this_device(c)) cudaFuncSetAttribute(prefill_attn_tc_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM_BYTES);
@@ -56,7 +56,7 @@ static int launch_prefill_paged_tc(const void* q, const void* k_cache, const voi
         if (first_use_on_this_device(c)) cudaFuncSetAttribute(prefill_attn_tc_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM_BYTES);
         prefill_attn_tc_kernel<__nv_bfloat16, true><<<grid, PT_THREADS, PT_SMEM_BYTES, stream>>>(qmap, kmap, vmap, p, pg);
     }
-    return check_launch("prefill_attention_paged(tcgen05)");
+    return check_launch("prefill_attention_paged(wgmma)");
 }
 
 }  // namespace sllm
@@ -90,7 +90,7 @@ extern "C" int sllm_prefill_attention_paged(const void* q, const void* k_cache, 
                                        softmax_scale * 1.4426950408889634f, num_prefill_seqs, max_prefill_len, num_prefill_tokens,
                                        nq, nkv, q_row_stride, cache_rows, pg, dtype, st);
     }
-    SLLM_REQUIRE(gen != 2, "prefill_attention_paged: SLLM_PREFILL_ATTN_GEN=2 but the shape is not covered by the tcgen05 kernel");
+    SLLM_REQUIRE(gen != 2, "prefill_attention_paged: SLLM_PREFILL_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
     PfPagedKV pk{block_table, seq_ids, prefill_prefix_lens, cur_layer, num_layers, block_size, max_blocks_per_seq};
     if (head_dim == 128) { SLLM_DISPATCH_DTYPE(dtype, return (launch_prefill_paged<T, 128>(q, k_cache, v_cache, o, prefill_seq_start_locs, prefill_seq_lens, softmax_scale, num_prefill_seqs, max_prefill_len, nq, nkv, q_row_stride, pk, st))); }
     else { SLLM_DISPATCH_DTYPE(dtype, return (launch_prefill_paged<T, 64>(q, k_cache, v_cache, o, prefill_seq_start_locs, prefill_seq_lens, softmax_scale, num_prefill_seqs, max_prefill_len, nq, nkv, q_row_stride, pk, st))); }

@@ -1,4 +1,4 @@
-// Causal varlen prefill attention, generation 2 (tcgen05 + TMA): host side of the packed-k/v variant.  The kernel is
+// Causal varlen prefill attention, generation 2 (TMA + wgmma): host side of the packed-k/v variant.  The kernel is
 // prefill_attn_tc_kernel.cuh; reference being replaced: swiftllm/worker/kernels/prefill_attn.py:9-139 and the
 // flash_attn_varlen_func call at swiftllm/worker/layers/transformer_layer.py:86-96.
 #include <mutex>
@@ -57,7 +57,7 @@ int launch_prefill_tc(const void* q, const void* k, const void* v, void* o, cons
                  "prefill_attention: cuTensorMapEncodeTiled failed");
     PtParams p;
     p.o = o; p.start_locs = start_locs; p.seq_lens = seq_lens; p.scale_log2e = scale_log2e; p.nq = nq; p.nkv = nkv;
-    dim3 grid((max_len + 2 * PT_BQ - 1) / (2 * PT_BQ), nq, num_seqs);
+    dim3 grid((max_len + PT_BQ - 1) / PT_BQ, nq, num_seqs);
     if (dtype == SLLM_F16) {
         static unsigned long long c = 0;
         if (first_use_on_this_device(c)) cudaFuncSetAttribute(prefill_attn_tc_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM_BYTES);
@@ -67,7 +67,7 @@ int launch_prefill_tc(const void* q, const void* k, const void* v, void* o, cons
         if (first_use_on_this_device(c)) cudaFuncSetAttribute(prefill_attn_tc_kernel<__nv_bfloat16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM_BYTES);
         prefill_attn_tc_kernel<__nv_bfloat16, false><<<grid, PT_THREADS, PT_SMEM_BYTES, stream>>>(qmap, kmap, vmap, p, PtPaged{});
     }
-    return check_launch("prefill_attention(tcgen05)");
+    return check_launch("prefill_attention(wgmma)");
 }
 
 }  // namespace sllm

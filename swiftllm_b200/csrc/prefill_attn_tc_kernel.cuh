@@ -1,4 +1,4 @@
-// Causal varlen prefill attention, generation 2 kernel: tcgen05 + TMA, two query tiles per CTA in ping-pong (sm_100a).
+// Causal varlen prefill attention, generation 2 kernel: TMA + wgmma, two consumer warpgroups per CTA (sm_90a).
 // Shared by prefill_attn_tc.cu (packed k/v of the batch) and prefill_attn_paged.cu (chunked prefill: K/V pages gathered
 // from the KV cache through the block table).
 //
@@ -6,17 +6,14 @@
 // swiftllm/worker/layers/transformer_layer.py:86-96.  head_dim 128, fp16/bf16; numerics per SURVEY.md Appendix A6
 // (fp32 scores, exp2 online softmax in fp32, P rounded to the storage dtype before P.V, o = h(acc / l)).
 //
-// CTA = (sequence, q head, 256 query rows) = two 128-row tiles A and B.  352 threads:
-//   warp 0/10   TMA producers: warp 0 loads Q (4 boxes of 128 rows x 64 d) once and then the K tiles, warp 10 the V tiles
+// CTA = (sequence, q head, 128 query rows).  384 threads:
+//   warp 0 / 1  TMA producers: warp 0 loads Q (2 boxes of 128 rows x 64 d) once and then the K tiles, warp 1 the V tiles
 //               (2 boxes of 64 x 64 per 64-token step) into separate 3-stage rings with their own mbarriers.
-//   warp 1      MMA issuer (one thread, polling):  S_X[128 x 64] = Q_X . K_j^T       (8 UMMAs, M=128 N=64 K=16)
-//                                                   O_X[128 x 128] += P_X . V_j       (4 UMMAs, M=128 N=128 K=16, B MN-major)
-//               S_A, S_B (64 TMEM columns each) and O_A, O_B (128 columns each) live in TMEM.
-//   warps 2-5   softmax of tile A, warps 6-9 softmax of tile B: thread = query row = TMEM lane.  Row max and row sum
-//               are thread-local (no shuffles); P (storage dtype) goes to shared memory as the A operand of the PV
-//               UMMA; O is rescaled in TMEM only when the running max grew by more than 2^8 ("lazy rescale": the
-//               reference point m_ref trails the true max, exact in the end because l uses the same reference).
-// While one tile's softmax runs on the CUDA cores the tensor pipe works on the other tile.
+//   warpgroups 1 and 2  query rows 0-63 and 64-127: S[64 x 64] = Q . K_j^T   (8 wgmma m64n64k16, both operands in shared
+//               memory), online softmax on the register tile (row max / sum over the 4 lanes of a quad), P rounded to
+//               the storage dtype as register A operands of O[64 x 128] += P . V_j   (4 wgmma m64n128k16, V MN-major).
+//               O is rescaled only when the running max grew by more than 2^8 ("lazy rescale": the reference point m_ref
+//               trails the true max, exact in the end because l uses the same reference).
 // Roofline: tensor-bound; FLOPs = 4 * nq * D * sum_i L_i (L_i + 1) / 2.
 #pragma once
 #include "tc_helpers.cuh"
@@ -26,21 +23,18 @@ namespace sllm {
 using namespace tc;
 
 constexpr int PT_D = 128;
-constexpr int PT_BQ = 128;                // rows per query tile (two tiles per CTA)
+constexpr int PT_BQ = 128;                // query rows per CTA (64 per consumer warpgroup)
 constexpr int PT_BK = 64;                 // kv tokens per pipeline step
 constexpr int PT_STAGES = 3;               // K and V rings (separate producers): two steps of prefetch ahead of the MMA
-constexpr int PT_THREADS = 352;            // warp 0 K+Q producer, 1 MMA, 2-5 softmax A, 6-9 softmax B, 10 V producer
-constexpr int PT_Q_BYTES = PT_BQ * PT_D * 2;          // 32 KiB per query tile ([half][128 rows][128 B])
+constexpr int PT_THREADS = 384;            // warpgroup 0: warp 0 Q+K producer, warp 1 V producer; warpgroups 1, 2: MMA + softmax
+constexpr int PT_Q_BYTES = PT_BQ * PT_D * 2;          // 32 KiB ([half][128 rows][128 B])
 constexpr int PT_KV_BYTES = PT_BK * PT_D * 2;         // 16 KiB per K (or V) tile ([half][64 rows][128 B])
-constexpr int PT_P_BYTES = PT_BQ * PT_BK * 2;         // 16 KiB per P tile ([128 rows][128 B])
-constexpr int PT_SMEM_BYTES = 2 * PT_Q_BYTES + 2 * PT_STAGES * PT_KV_BYTES + 4 * PT_P_BYTES + 1024;   // P double buffered per tile
-constexpr int PT_TMEM_COLS = 512;         // S_A 0..63, S_B 64..127, O_A 128..255, O_B 256..383
+constexpr int PT_SMEM_BYTES = PT_Q_BYTES + 2 * PT_STAGES * PT_KV_BYTES + 1024;
 constexpr float PT_RESCALE_THRESHOLD = 8.0f;          // log2 units
 
 struct PtBarriers {
     uint64_t q_full;
     uint64_t k_full[PT_STAGES], k_empty[PT_STAGES], v_full[PT_STAGES], v_empty[PT_STAGES];
-    uint64_t s_full[2], s_empty[2], p_full[2][2], p_empty[2][2];      // P: [tile][buffer]
 };
 
 struct PtParams {
@@ -57,57 +51,34 @@ struct PtPaged {
 };
 constexpr int PT_PAGE = 16;               // tokens per KV page (PAGED only)
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                   "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                   "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-                 :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-                    "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-                    "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-                    "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // PAGED = false: K/V tiles come from the packed k/v rows of the batch (the reference's contract).
 // PAGED = true (chunked prefill, SURVEY.md §8 f-1): the chunk's queries sit at positions prefix .. prefix + len - 1 of
 // their sequence; every 64-token K/V step is gathered from four 16-token pages of the KV cache through the block
 // table (lanes 0-3 of the producer warp issue the two d-half boxes of one page each), landing in the SAME
-// [half][64 rows][128 B] layout, so the MMA issuer and its descriptors are shared by both variants.
+// [half][64 rows][128 B] layout, so the consumer warpgroups and their descriptors are shared by both variants.
 template <typename T, bool PAGED>
 __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap qmap,
                                                                         const __grid_constant__ CUtensorMap kmap,
                                                                         const __grid_constant__ CUtensorMap vmap,
                                                                         const PtParams p, const PtPaged pg) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint8_t* q_sm = smem;                                       // [2 tiles][2 halves][128 rows][128 B]
-    uint8_t* k_sm = q_sm + 2 * PT_Q_BYTES;                      // [stage][2 halves][64 rows][128 B]
+    uint8_t* q_sm = smem;                                       // [2 halves][128 rows][128 B]
+    uint8_t* k_sm = q_sm + PT_Q_BYTES;                          // [stage][2 halves][64 rows][128 B]
     uint8_t* v_sm = k_sm + PT_STAGES * PT_KV_BYTES;
-    uint8_t* p_sm = v_sm + PT_STAGES * PT_KV_BYTES;             // [2 tiles][2 buffers][128 rows][128 B]
-    uint8_t* misc = p_sm + 4 * PT_P_BYTES;
-    PtBarriers* bars = reinterpret_cast<PtBarriers*>(misc);
-    uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(misc + 512);
+    PtBarriers* bars = reinterpret_cast<PtBarriers*>(v_sm + PT_STAGES * PT_KV_BYTES);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int qblk = gridDim.x - 1 - blockIdx.x;                // latest (heaviest) query blocks first
     const int head = blockIdx.y, seq = blockIdx.z;
     const int len = p.seq_lens[seq];                            // query rows of this sequence in the batch
-    const int q0 = qblk * 2 * PT_BQ;
+    const int q0 = qblk * PT_BQ;
     if (q0 >= len) return;
     const int tok0 = p.start_locs[seq];
     const int kvh = head / (p.nq / p.nkv);
     const int pre = PAGED ? pg.prefix_lens[seq] : 0;            // position of query row 0 within its sequence
     const int kvlen = pre + len;
-    const bool active_b = q0 + PT_BQ < len;
-    const int nkt_a = (min(kvlen, pre + q0 + PT_BQ) + PT_BK - 1) / PT_BK;   // kv steps tile A takes part in
-    const int nkt_b = active_b ? (min(kvlen, pre + q0 + 2 * PT_BQ) + PT_BK - 1) / PT_BK : 0;
-    const int nkt = max(nkt_a, nkt_b);
+    // kv steps of the CTA; both warpgroups run all of them (the last one may be fully masked for warpgroup 1's rows)
+    const int nkt = (min(kvlen, pre + q0 + PT_BQ) + PT_BK - 1) / PT_BK;
 
     if constexpr (PAGED) {
         // page slots that a tail step never loads must hold finite data (their P columns are exactly 0)
@@ -118,21 +89,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
     if (tid == 0) {
         mbar_init(smem_u32(&bars->q_full), 1);
         for (int i = 0; i < PT_STAGES; i++) {
-            mbar_init(smem_u32(&bars->k_full[i]), 1); mbar_init(smem_u32(&bars->k_empty[i]), 1);
-            mbar_init(smem_u32(&bars->v_full[i]), 1); mbar_init(smem_u32(&bars->v_empty[i]), 1);
-        }
-        for (int i = 0; i < 2; i++) {
-            mbar_init(smem_u32(&bars->s_full[i]), 1); mbar_init(smem_u32(&bars->s_empty[i]), 128);
-            for (int b = 0; b < 2; b++) { mbar_init(smem_u32(&bars->p_full[i][b]), 128); mbar_init(smem_u32(&bars->p_empty[i][b]), 1); }
+            mbar_init(smem_u32(&bars->k_full[i]), 1); mbar_init(smem_u32(&bars->k_empty[i]), 256);
+            mbar_init(smem_u32(&bars->v_full[i]), 1); mbar_init(smem_u32(&bars->v_empty[i]), 256);
         }
         mbar_fence_init();
         tma_prefetch_desc(&qmap); tma_prefetch_desc(&kmap); tma_prefetch_desc(&vmap);
     }
-    if (warp == 1) tmem_alloc<PT_TMEM_COLS>(smem_u32(tmem_base_s));
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_base_s;
 
     // PAGED producer (one whole warp per ring): step j = pages 4j .. 4j+3 of the sequence.  The four block-table
     // entries of the NEXT step are fetched before this step's stage is waited for; lane 0 arms the mbarrier with the
@@ -168,11 +131,9 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
         // =========================================================== TMA producer: Q once, then the K tiles
         if (lane == 0) {
             const uint32_t qbar = smem_u32(&bars->q_full);
-            mbar_arrive_expect_tx(qbar, 2 * PT_Q_BYTES);
-            for (int x = 0; x < 2; x++)
-                for (int h = 0; h < 2; h++)
-                    tma_load_2d(smem_u32(q_sm + x * PT_Q_BYTES + h * (PT_Q_BYTES / 2)), &qmap, qbar, head * PT_D + h * 64,
-                                tok0 + q0 + x * PT_BQ);
+            mbar_arrive_expect_tx(qbar, PT_Q_BYTES);
+            for (int h = 0; h < 2; h++)
+                tma_load_2d(smem_u32(q_sm + h * (PT_Q_BYTES / 2)), &qmap, qbar, head * PT_D + h * 64, tok0 + q0);
             if constexpr (!PAGED) {
                 for (int j = 0; j < nkt; j++) {
                     const int st = j % PT_STAGES;
@@ -185,7 +146,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
             }
         }
         if constexpr (PAGED) paged_producer(kmap, k_sm, bars->k_full, bars->k_empty);
-    } else if (warp == 10) {
+    } else if (warp == 1) {
         // =========================================================== TMA producer: the V tiles (independent of K's progress)
         if constexpr (PAGED) {
             paged_producer(vmap, v_sm, bars->v_full, bars->v_empty);
@@ -199,215 +160,110 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
                 tma_load_2d(smem_u32(v_sm + st * PT_KV_BYTES + PT_KV_BYTES / 2), &vmap, vb, kvh * PT_D + 64, tok0 + j * PT_BK);
             }
         }
-    } else if (warp == 1) {
-        // =========================================================== MMA issuer: the whole warp runs the polling loop
-        // converged (votes make the control flow provably uniform); one elected lane issues the UMMAs and commits.
-        {
-            constexpr uint32_t IDESC_S = make_instr_desc(128, PT_BK, UmmaFmt<T>::value, 0, 0);
-            constexpr uint32_t IDESC_O = make_instr_desc(128, PT_D, UmmaFmt<T>::value, 0, 1);      // B = V, MN-major
-            constexpr uint32_t FULL = 0xffffffffu;
-            const uint32_t tm = __shfl_sync(FULL, tmem, 0);
-            // Descriptor bases are loop invariants; per UMMA only the 14-bit address field (16-byte units, low word)
-            // advances by a compile-time constant (all tiles live below 256 KiB, so no carry into the LBO field).
-            const uint64_t dq0 = make_smem_desc(smem_u32(q_sm), 16, 1024);
-            const uint64_t dk0 = make_smem_desc(smem_u32(k_sm), 16, 1024);
-            const uint64_t dv0 = make_smem_desc(smem_u32(v_sm), PT_KV_BYTES / 2, 1024);             // MN-major: LBO = d-half stride
-            const uint64_t dp0 = make_smem_desc(smem_u32(p_sm), 16, 1024);
-            mbar_wait(smem_u32(&bars->q_full), 0);
-            int js = 0, jpa = 0, jpb = 0;
-            uint32_t spins = 0;
-            while (jpa < nkt_a || jpb < nkt_b) {
-                bool progressed = false;
-                if (js < nkt) {      // S_A(js), S_B(js)
-                    const int st = js % PT_STAGES;
-                    const bool ua = js < nkt_a, ub = js < nkt_b;
-                    const uint32_t spar = (js & 1) ^ 1;
-                    const bool ready = mbar_test_wait(smem_u32(&bars->k_full[st]), (js / PT_STAGES) & 1) &&
-                                       (!ua || mbar_test_wait(smem_u32(&bars->s_empty[0]), spar)) &&
-                                       (!ub || mbar_test_wait(smem_u32(&bars->s_empty[1]), spar));
-                    if (__all_sync(FULL, ready)) {
-                        tc_fence_after();
-                        if (elect_one()) {
-                            const uint64_t kd = dk0 + (uint64_t)((st * PT_KV_BYTES) >> 4);
+    } else if (warp >= 4) {
+        // =========================================================== consumer warpgroup x: query rows 64 x .. 64 x + 63
+        // Thread (warp w of the group, lane l) owns rows rr = 16 w + l / 4 + 8 hi (hi in {0, 1}) and, of every 8-column
+        // group i, columns 8 i + 2 (l % 4) + {0, 1} of the S and O tiles (see tc_helpers.cuh).
+        const int x = (warp >> 2) - 1;
+        const int rbase = 16 * (warp & 3) + (lane >> 2);
+        const int qi0 = q0 + 64 * x + rbase;              // query index (within the sequence) of the thread's row hi = 0
+        const int cb = 2 * (lane & 3);
+        // descriptor bases (all tiles live below 256 KiB, so adding 16-byte units to the low word never carries)
+        const uint64_t dq0 = make_smem_desc(smem_u32(q_sm + x * 64 * 128), 16, 1024);
+        const uint64_t dk0 = make_smem_desc(smem_u32(k_sm), 16, 1024);
+        const uint64_t dv0 = make_smem_desc(smem_u32(v_sm), PT_KV_BYTES / 2, 1024);      // MN-major: LBO = d-half stride
+        float o[64];
 #pragma unroll
-                            for (int x = 0; x < 2; x++) {
-                                if (x == 0 ? ua : ub) {
-                                    const uint64_t qd = dq0 + (uint64_t)((x * PT_Q_BYTES) >> 4);
+        for (int i = 0; i < 64; i++) o[i] = 0.f;
+        float m_ref[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+        const float c = p.scale_log2e;
+        mbar_wait(smem_u32(&bars->q_full), 0);
+        for (int j = 0; j < nkt; j++) {
+            const int st = j % PT_STAGES;
+            // ---- S = Q . K_j^T
+            mbar_wait(smem_u32(&bars->k_full[st]), (j / PT_STAGES) & 1);
+            float sc[32];
+            {
+                const uint64_t kd = dk0 + (uint64_t)((st * PT_KV_BYTES) >> 4);
+                wgmma_fence();
 #pragma unroll
-                                    for (int ks = 0; ks < 8; ks++)      // 16 d per UMMA; d-half = ks / 4
-                                        umma_ss(tm + x * 64, qd + (uint64_t)(((ks >> 2) * (PT_Q_BYTES / 2) + (ks & 3) * 32) >> 4),
-                                                kd + (uint64_t)(((ks >> 2) * (PT_KV_BYTES / 2) + (ks & 3) * 32) >> 4), IDESC_S, ks > 0);
-                                    umma_commit(smem_u32(&bars->s_full[x]));
-                                }
-                            }
-                            umma_commit(smem_u32(&bars->k_empty[st]));
-                        }
-                        __syncwarp();
-                        js++;
-                        progressed = true;
-                    }
-                }
-#pragma unroll
-                for (int x = 0; x < 2; x++) {     // PV_X(jp[x])
-                    const int j = x == 0 ? jpa : jpb;
-                    const int nkx = x == 0 ? nkt_a : nkt_b;
-                    if (j < nkx && j < js) {
-                        const int st = j % PT_STAGES;
-                        const int pb = j & 1;
-                        const bool ready = mbar_test_wait(smem_u32(&bars->p_full[x][pb]), (j >> 1) & 1) &&
-                                           mbar_test_wait(smem_u32(&bars->v_full[st]), (j / PT_STAGES) & 1);
-                        if (__all_sync(FULL, ready)) {
-                            tc_fence_after();
-                            // the V stage is free once every tile that uses it has issued its PV
-                            const int jo = x == 0 ? jpb : jpa, nko = x == 0 ? nkt_b : nkt_a;
-                            const bool release_v = j >= nko || jo > j;
-                            if (elect_one()) {
-                                const uint64_t vd = dv0 + (uint64_t)((st * PT_KV_BYTES) >> 4);
-                                const uint64_t pd = dp0 + (uint64_t)(((x * 2 + pb) * PT_P_BYTES) >> 4);
-#pragma unroll
-                                for (int kt = 0; kt < 4; kt++)       // 16 tokens per UMMA
-                                    umma_ss(tm + 128 + x * 128, pd + (uint64_t)((kt * 32) >> 4), vd + (uint64_t)((kt * 2048) >> 4), IDESC_O,
-                                            (j > 0 || kt > 0) ? 1u : 0u);
-                                umma_commit(smem_u32(&bars->p_empty[x][pb]));
-                                if (release_v) umma_commit(smem_u32(&bars->v_empty[st]));
-                            }
-                            __syncwarp();
-                            if (x == 0) jpa++; else jpb++;
-                            progressed = true;
-                        }
-                    }
-                }
-                if (progressed) spins = 0;
-                else if (++spins > (1u << 24)) {
-                    if (lane == 0) printf("sllm: prefill MMA watchdog (block %d,%d,%d js=%d jpA=%d jpB=%d)\n", blockIdx.x, blockIdx.y, blockIdx.z, js, jpa, jpb);
-                    __trap();
-                }
+                for (int ks = 0; ks < 8; ks++)      // 16 d per wgmma; d-half = ks / 4
+                    wgmma_m64n64k16_ss<T, 0, 0>(sc, dq0 + (uint64_t)(((ks >> 2) * (PT_Q_BYTES / 2) + (ks & 3) * 32) >> 4),
+                                                kd + (uint64_t)(((ks >> 2) * (PT_KV_BYTES / 2) + (ks & 3) * 32) >> 4), ks > 0);
+                wgmma_commit();
+                wgmma_wait<0>();
             }
-        }
-    } else {
-        // =========================================================== softmax warps: group x = 0 (tile A) / 1 (tile B)
-        const int x = (warp - 2) >> 2;
-        const int nk_mine = x == 0 ? nkt_a : nkt_b;
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;                 // row within the tile = TMEM lane
-        const int qi = q0 + x * PT_BQ + row;              // query index within the sequence
-        const uint32_t tlane = (uint32_t)(quad * 32) << 16;
-        const uint32_t s_addr = tmem + tlane + x * 64;
-        const uint32_t o_addr = tmem + tlane + 128 + x * 128;
-        float m_ref = -INFINITY, l = 0.f;
-        for (int j = 0; j < nk_mine; j++) {
-            mbar_wait(smem_u32(&bars->s_full[x]), j & 1);
-            tc_fence_after();
-            uint32_t r0[32], r1[32];
-            tmem_ld32(s_addr, r0);
-            tmem_ld32(s_addr + 32, r1);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(smem_u32(&bars->s_empty[x]));              // S buffer free: the next S UMMAs may overwrite it
+            mbar_arrive(smem_u32(&bars->k_empty[st]));
 
+            // ---- mask, row max over the quad, lazy rescale
             const int c0 = j * PT_BK;
-            const bool need_mask = c0 + PT_BK - 1 > pre + q0 + x * PT_BQ || c0 + PT_BK > kvlen;
-            // column c0+i is visible iff c0+i <= pre+qi and c0+i < kvlen  <=>  i <= lim   (branch-free selects)
-            const int lim = min(pre + qi, kvlen - 1) - c0;
-            float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;   // 4 independent chains
-            if (need_mask) {
+            const bool need_mask = c0 + PT_BK - 1 > pre + q0 + 64 * x || c0 + PT_BK > kvlen;
+            float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int i = 0; i < 32; i++) r0[i] = i <= lim ? r0[i] : 0xff800000u;        // -inf
-            }
+            for (int hi = 0; hi < 2; hi++) {
+                // column c0+i is visible iff c0+i <= pre+qi and c0+i < kvlen  <=>  i <= lim   (branch-free selects)
+                const int lim = min(pre + qi0 + 8 * hi, kvlen - 1) - c0;
 #pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                mx0 = fmaxf(mx0, __uint_as_float(r0[i])); mx1 = fmaxf(mx1, __uint_as_float(r0[i + 1]));
-                mx2 = fmaxf(mx2, __uint_as_float(r0[i + 2])); mx3 = fmaxf(mx3, __uint_as_float(r0[i + 3]));
-            }
-            if (need_mask) {
+                for (int i = 0; i < 8; i++)
 #pragma unroll
-                for (int i = 0; i < 32; i++) r1[i] = i + 32 <= lim ? r1[i] : 0xff800000u;
-            }
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                mx0 = fmaxf(mx0, __uint_as_float(r1[i])); mx1 = fmaxf(mx1, __uint_as_float(r1[i + 1]));
-                mx2 = fmaxf(mx2, __uint_as_float(r1[i + 2])); mx3 = fmaxf(mx3, __uint_as_float(r1[i + 3]));
-            }
-            const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));       // max of the RAW scores (scale > 0 commutes with max)
-            const float m_new = fmaxf(m_ref, mx * p.scale_log2e);
-            // Lazy rescale.  The decision is per row, but tcgen05.ld/st are warp-collective (.sync.aligned): vote, and
-            // let rows that do not need it take part with alpha = 1.
-            const bool need = m_new > m_ref + PT_RESCALE_THRESHOLD;   // always true on the first tile (m_ref = -inf)
-            if (j > 0 && __any_sync(0xffffffffu, need)) {
-                // O must be stable: wait until PV(j-1) of this tile has completed, then rescale this thread's row
-                mbar_wait(smem_u32(&bars->p_empty[x][(j - 1) & 1]), ((j - 1) >> 1) & 1);
-                const float alpha = need ? fast_exp2_tc(m_ref - m_new) : 1.0f;
-                l *= alpha;
-                tc_fence_after();
-#pragma unroll
-                for (int cc = 0; cc < 4; cc++) {
-                    uint32_t t[32];
-                    tmem_ld32(o_addr + cc * 32, t);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; i++) t[i] = __float_as_uint(__uint_as_float(t[i]) * alpha);
-                    tmem_st32(o_addr + cc * 32, t);
-                }
-                tmem_st_wait();
-                tc_fence_before();
-            }
-            if (need) m_ref = m_new;
-            // P buffer (j & 1) was last read by PV(j-2)
-            const int pb = j & 1;
-            if (j >= 2) mbar_wait(smem_u32(&bars->p_empty[x][pb]), ((j - 2) >> 1) & 1);
-            // p = exp2(s*c - m_ref) (<= 2^8), row sum in fp32, P row -> shared memory ([128 rows][128 B], SWIZZLE_128B)
-            float ls0 = 0.f, ls1 = 0.f;
-            const float neg_m = -m_ref, c = p.scale_log2e;
-            uint8_t* prow = p_sm + (x * 2 + pb) * PT_P_BYTES + row * 128;
-#pragma unroll
-            for (int ch = 0; ch < 8; ch++) {                       // 8 chunks of 8 tokens
-                uint32_t w[4];
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int i = ch * 8 + e * 2;                  // token pair (i, i+1) of this 64-token step
-                    const float a = fast_exp2_tc(fmaf(__uint_as_float(i < 32 ? r0[i] : r1[i - 32]), c, neg_m));
-                    const float b = fast_exp2_tc(fmaf(__uint_as_float(i + 1 < 32 ? r0[i + 1] : r1[i + 1 - 32]), c, neg_m));
-                    ls0 += a; ls1 += b;
-                    typename Traits<T>::T2 v2 = Traits<T>::from_f2(make_float2(a, b));
-                    w[e] = *reinterpret_cast<uint32_t*>(&v2);
-                }
-                *reinterpret_cast<uint4*>(prow + ((ch ^ (row & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-            l += ls0 + ls1;
-            fence_proxy_async();
-            mbar_arrive(smem_u32(&bars->p_full[x][pb]));
-        }
-        if (nk_mine > 0) {
-            // ---- epilogue: O / l -> global (row qi of this head), only rows inside the sequence
-            mbar_wait(smem_u32(&bars->p_empty[x][(nk_mine - 1) & 1]), ((nk_mine - 1) >> 1) & 1);   // PV(last) done => all done
-            tc_fence_after();
-            const float inv = 1.0f / l;
-            T* orow = reinterpret_cast<T*>(p.o) + ((int64_t)(tok0 + qi) * p.nq + head) * PT_D;
-#pragma unroll
-            for (int cc = 0; cc < 4; cc++) {
-                uint32_t t[32];
-                tmem_ld32(o_addr + cc * 32, t);
-                tmem_ld_wait();
-                if (qi < len) {
-#pragma unroll
-                    for (int v = 0; v < 4; v++) {
-                        uint32_t w[4];
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            typename Traits<T>::T2 v2 = Traits<T>::from_f2(make_float2(__uint_as_float(t[v * 8 + e * 2]) * inv,
-                                                                                        __uint_as_float(t[v * 8 + e * 2 + 1]) * inv));
-                            w[e] = *reinterpret_cast<uint32_t*>(&v2);
-                        }
-                        *reinterpret_cast<uint4*>(orow + cc * 32 + v * 8) = make_uint4(w[0], w[1], w[2], w[3]);
+                    for (int e = 0; e < 2; e++) {
+                        float& v = sc[4 * i + 2 * hi + e];
+                        if (need_mask && 8 * i + cb + e > lim) v = -INFINITY;
+                        mx[hi] = fmaxf(mx[hi], v);
                     }
+                mx[hi] = fmaxf(mx[hi], __shfl_xor_sync(0xffffffffu, mx[hi], 1));
+                mx[hi] = fmaxf(mx[hi], __shfl_xor_sync(0xffffffffu, mx[hi], 2));
+                const float m_new = fmaxf(m_ref[hi], mx[hi] * c);       // max of the RAW scores (scale > 0 commutes with max)
+                if (m_new > m_ref[hi] + PT_RESCALE_THRESHOLD) {         // always true on the first step (m_ref = -inf)
+                    const float alpha = fast_exp2_tc(m_ref[hi] - m_new);
+                    l[hi] *= alpha;
+#pragma unroll
+                    for (int i = 0; i < 16; i++) { o[4 * i + 2 * hi] *= alpha; o[4 * i + 2 * hi + 1] *= alpha; }
+                    m_ref[hi] = m_new;
+                }
+            }
+            // ---- p = exp2(s*c - m_ref) (<= 2^8), row sums in fp32, P -> register A fragments (storage dtype)
+            uint32_t pa[4][4];
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+#pragma unroll
+                for (int hi = 0; hi < 2; hi++) {
+                    const float a = fast_exp2_tc(fmaf(sc[4 * i + 2 * hi], c, -m_ref[hi]));
+                    const float b = fast_exp2_tc(fmaf(sc[4 * i + 2 * hi + 1], c, -m_ref[hi]));
+                    l[hi] += a + b;
+                    typename Traits<T>::T2 v2 = Traits<T>::from_f2(make_float2(a, b));
+                    pa[i >> 1][(i & 1) * 2 + hi] = *reinterpret_cast<uint32_t*>(&v2);
+                }
+            // ---- O += P . V_j
+            mbar_wait(smem_u32(&bars->v_full[st]), (j / PT_STAGES) & 1);
+            {
+                const uint64_t vd = dv0 + (uint64_t)((st * PT_KV_BYTES) >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int kt = 0; kt < 4; kt++)       // 16 tokens per wgmma
+                    wgmma_m64n128k16_rs<T, 1>(o, pa[kt], vd + (uint64_t)((kt * 2048) >> 4), 1);
+                wgmma_commit();
+                wgmma_wait<0>();
+            }
+            mbar_arrive(smem_u32(&bars->v_empty[st]));
+        }
+        // ---- epilogue: O / l -> global (rows inside the sequence)
+#pragma unroll
+        for (int hi = 0; hi < 2; hi++) {
+            l[hi] += __shfl_xor_sync(0xffffffffu, l[hi], 1);
+            l[hi] += __shfl_xor_sync(0xffffffffu, l[hi], 2);
+            const int qi = qi0 + 8 * hi;
+            if (qi < len) {
+                const float inv = 1.0f / l[hi];
+                T* orow = reinterpret_cast<T*>(p.o) + ((int64_t)(tok0 + qi) * p.nq + head) * PT_D;
+#pragma unroll
+                for (int i = 0; i < 16; i++) {
+                    typename Traits<T>::T2 v2 = Traits<T>::from_f2(make_float2(o[4 * i + 2 * hi] * inv, o[4 * i + 2 * hi + 1] * inv));
+                    *reinterpret_cast<typename Traits<T>::T2*>(orow + 8 * i + cb) = v2;
                 }
             }
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<PT_TMEM_COLS>(tmem);
 }
 
 // host (prefill_attn_tc.cu): cached cuTensorMapEncodeTiled of a [rows, cols] 16-bit tensor, boxes of (64 cols x box_rows)

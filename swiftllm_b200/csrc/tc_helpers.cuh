@@ -1,9 +1,11 @@
-// Blackwell (sm_100a) primitives used by the tcgen05/TMA kernels: mbarrier, TMA tensor loads, UMMA shared-memory
-// and instruction descriptors, tcgen05.mma / commit / ld, TMEM allocation.  Inline PTX only.
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptors" (cross-checked against the field
-// definitions in CUTLASS cute/arch/mma_sm100_desc.hpp) and were validated on hardware with probes/umma_probe.cu.
+// Hopper (sm_90a) primitives used by the TMA + wgmma kernels: mbarrier, TMA tensor loads, wgmma shared-memory
+// descriptors and the warpgroup MMA itself (fp32 accumulators in registers).  Inline PTX only.
+// Descriptor bit layouts follow the PTX ISA "warpgroup-level matrix shared memory layout" section (matrix descriptor
+// format for wgmma).
 #pragma once
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -44,8 +46,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 
 // ------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -64,77 +64,91 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B.  K-major operand: rows of 128 B (64 x 16-bit along K), 8-row
-// atoms 1 KiB apart by `sbo` bytes (LBO unused).  MN-major operand: atoms of 8 K-rows x 64 MN-elements; `lbo` =
-// byte distance between MN-adjacent atoms, `sbo` = byte distance between K-adjacent atoms.
+// ------------------------------------------------------------------ wgmma descriptors
+// Shared-memory matrix descriptor, SWIZZLE_128B (1 KiB-aligned atoms).  K-major operand: rows of 128 B (64 x 16-bit
+// along K), 8-row atoms `sbo` bytes apart (LBO unused); a K step of 16 elements advances the start address by 32 B.
+// MN-major operand: atoms of 8 K-rows x 64 MN-elements; `lbo` = byte distance between MN-adjacent atoms, `sbo` = byte
+// distance between K-adjacent atoms.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;      // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;      // layout type: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;      // layout type: SWIZZLE_128B
     return d;
 }
-// Instruction descriptor for kind::f16: fp32 accumulator, A/B both fp16 (fmt 0) or bf16 (fmt 1).
-__host__ __device__ constexpr uint32_t make_instr_desc(int M, int N, int fmt, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)a_mn_major << 15) |
-           ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-template <typename T> struct UmmaFmt;
-template <> struct UmmaFmt<__half> { static constexpr int value = 0; };
-template <> struct UmmaFmt<__nv_bfloat16> { static constexpr int value = 1; };
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all previously issued MMAs of this thread arrive on `bar` when they complete (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// ------------------------------------------------------------------ wgmma (issued by all 128 threads of a warpgroup)
+// Accumulator fragment of an m64nN tile, thread t = 32 w + l of the warpgroup: d[4i + e] holds row 16 w + l / 4 + 8 (e >> 1)
+// and column 8 i + 2 (l % 4) + (e & 1).  The register A fragment of m64k16 uses the same (row, column) pairs for its
+// four 32-bit registers (columns 0..7 then 8..15), so an accumulator tile converts to A operands register for register.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D (+)= A * B with A and B in shared memory (_ss) or A in registers (_rs); TA / TB = 1: that operand is MN-major
+// (transposed), 16-bit types only
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n8k16_ss(float (&d)[4], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (std::is_same<T, __half>::value)
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %6, 0;\n wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 "
+                     "{%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+    else
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %6, 0;\n wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+                     "{%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
 }
 
-// ------------------------------------------------------------------ TMEM
-template <int COLS> __device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {      // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16_ss(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (std::is_same<T, __half>::value)
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %10, 0;\n wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+    else
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %10, 0;\n wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
 }
-template <int COLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {       // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// 32 lanes x N consecutive 32-bit columns; thread t of the warp reads TMEM lane (lane base of taddr) + t
-template <int N> __device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t (&r)[N]);
-template <> __device__ __forceinline__ void tmem_ld<4>(uint32_t taddr, uint32_t (&r)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr));
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (std::is_same<T, __half>::value)
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
+    else
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
 }
-template <> __device__ __forceinline__ void tmem_ld<8>(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
+
+template <typename T, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (std::is_same<T, __half>::value)
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %69, 0;\n wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, %70;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB) : "memory");
+    else
+        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %69, 0;\n wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, %70;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB) : "memory");
 }
-template <> __device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                   "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(taddr));
-}
+
 
 __device__ __forceinline__ float fast_exp2_tc(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// One lane of a CONVERGED warp.  Issuing tcgen05.mma from `if (elect_one())` inside warp-uniform control flow lets ptxas
-// keep the descriptors in uniform registers; under a plain `if (lane == 0)` it wraps every UTCHMMA in a
-// uniformisation loop (~14 extra instructions per MMA, measured in profiles/).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xffffffff;\n selp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
-    return pred != 0;
 }
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {

@@ -1,5 +1,5 @@
 """Engine configuration.  The first nine fields and their CLI flags are the reference's
-(swiftllm/engine_config.py:4-84); the trailing fields (with defaults) are additions for the B200 data plane."""
+(swiftllm/engine_config.py:4-84); the trailing fields (with defaults) are additions for the H100 data plane."""
 import argparse
 import dataclasses
 
@@ -38,15 +38,14 @@ class EngineConfig:
     fused_allreduce: object = None
     # TP: shard lm_head by vocabulary rows (each rank computes logits of V/tp_size tokens; the greedy token is found with one
     # tiny all-gather of per-rank (max logit, argmax) pairs) instead of replicating the 1 GB matrix on every rank.
-    # SURVEY.md §8 f-3.  None = automatic: sharded whenever tp_size > 1 and divides the vocabulary (measured on B200, decode
-    # batch 256: -0.10 / -0.15 / -0.20 ms per step at tp 2 / 4 / 8, profiles/r2_tp_sweep_*.jsonl).
+    # SURVEY.md §8 f-3.  None = automatic: sharded whenever tp_size > 1 and divides the vocabulary.
     shard_lm_head: object = None
     # pure-decode steps: rotary embedding + KV store of the new rows in ONE launch per layer instead of two.
     # Bit-identical to the two kernels (tests/test_decode_fusion_gpu.py); one launch less per layer.
     fuse_rotary_store: bool = True
     # swap in / out with device-resident id lists and one gather/scatter kernel over the pinned, mapped swap space (no host
-    # syncs) instead of `.tolist()` + cudaMemcpyAsync per run (SURVEY.md §8 f-4).  Needs pin_swap_space.  Validated on B200
-    # (tests/test_swap_device_gpu.py); opt-in: its copy speed (SM loads / stores over PCIe) against the DMA path is unmeasured.
+    # syncs) instead of `.tolist()` + cudaMemcpyAsync per run (SURVEY.md §8 f-4).  Needs pin_swap_space.  Tested by
+    # tests/test_swap_device_gpu.py; opt-in: its copy speed (SM loads / stores over PCIe) against the DMA path is unmeasured.
     device_swap: bool = False
     # swap copies run on a dedicated copy stream (SURVEY.md §8 f-4): swap_in_seqs / swap_out_seqs return as soon as the block
     # tables are updated and the copy is enqueued; the next forward waits for it on the device right before its first KV-cache

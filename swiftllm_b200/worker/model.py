@@ -7,7 +7,7 @@
 
 and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).
 
-B200-first host path (SURVEY.md §8 f-2): all per-step metadata travels in ONE pinned staging buffer and one
+Host path (SURVEY.md §8 f-2): all per-step metadata travels in ONE pinned staging buffer and one
 H2D copy (the reference issues ~6 small copies, model.py:272-297); block allocation is one sync-free kernel
 (three syncs + torch.nonzero in the reference, block_manager.py:50,70,75); pure-decode steps can be replayed
 from a CUDA graph; the only sync of a step is the final `.tolist()` of the sampled tokens.
@@ -125,9 +125,8 @@ class LlamaModel:
         want_fused = getattr(self.engine_config, "fused_allreduce", None)
         explicit = want_fused is not None
         if want_fused is None:
-            # measured on B200 / NVSwitch (profiles/r2_tp_sweep_*.jsonl), decode batch 256 x 4096:
-            #   tp 2, 4: one-shot peer-memory kernel (14 / 21 us per exchange vs NCCL 22 / 30 us + the add/norm launch)
-            #   tp 8:    row-owner kernel with in-switch reduction and broadcast (24.6 us vs NCCL 33.7 + 3.2 us)
+            #   tp 2, 4: one-shot peer-memory kernel
+            #   tp 8:    row-owner kernel with in-switch reduction and broadcast (falls back to peer memory, then NCCL)
             candidates = [True] if 2 <= self.tp_size <= 4 else (["two_shot_nvls", "two_shot"] if self.tp_size == 8 else [])
         else:
             candidates = [want_fused] if want_fused else []

@@ -11,16 +11,16 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "slow_cpu: CPU test that takes tens of seconds")
     config.addinivalue_line("markers", "pending_gpu: GPU test of code that has not run on hardware yet; skipped unless "
-                                       "SLLM_RUN_PENDING=1 (no test carries it at the moment: everything has run on a B200)")
+                                       "SLLM_RUN_PENDING=1 (no test carries it at the moment)")
 
 
 def pytest_collection_modifyitems(config, items):
     """Tests of kernels that have never run on a GPU must not be able to turn the validated suite red (the driver runs
-    `-m gpu -x`).  They are opted into with SLLM_RUN_PENDING=1 (scripts/gpu_validate_pending.sh) and lose the marker once
-    they have passed on a B200."""
+    `-m gpu -x`).  They are opted into with SLLM_RUN_PENDING=1 and lose the marker once
+    they have passed on an H100."""
     import torch
     lib_built = os.path.exists(os.path.join(ROOT, "swiftllm_b200", "libswiftllm_b200.so"))
     if not torch.cuda.is_available():

@@ -96,8 +96,8 @@ def test_no_silent_fallback_without_cuda():
 
 
 def test_validated_kernels_still_have_their_validated_instruction_streams():
-    """profiles/r2_validated_kernels.json (r1_... before round 2) holds a hash of the (normalised) SASS of every kernel as it last ran `pytest -m gpu`,
-    smoke() and bench.py on a B200.  Refactoring a kernel's source without a GPU at hand (templates, shared headers) is only safe
+    """profiles/validated_kernels.json holds a hash of the (normalised) SASS of every kernel as it last ran `pytest -m gpu`,
+    smoke() and bench.py on an H100.  Refactoring a kernel's source without a GPU at hand (templates, shared headers) is only safe
     if the instruction stream it compiles to is unchanged - or the change was reviewed and listed under "equivalent".  A kernel that
     no longer matches must be re-validated on a GPU and the manifest regenerated (scripts/sass_diff.py)."""
     import hashlib
@@ -108,9 +108,7 @@ def test_validated_kernels_still_have_their_validated_instruction_streams():
     import pytest
     if shutil.which("cuobjdump") is None or shutil.which("nvcc") is None:
         pytest.skip("CUDA toolkit not on PATH")
-    path = os.path.join(ROOT, "profiles", "r2_validated_kernels.json")
-    if not os.path.exists(path):
-        path = os.path.join(ROOT, "profiles", "r1_validated_kernels.json")
+    path = os.path.join(ROOT, "profiles", "validated_kernels.json")
     man = json.load(open(path))
     nvcc = subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout
     if man["nvcc"] not in nvcc:

@@ -3,7 +3,7 @@
   sllm_prefill_attention_paged    both kernel generations vs the fp64 definition; with prefix 0 vs sllm_prefill_attention
   LlamaModel.forward(..., prefill_prefix_lens_list=...)   chunked == whole-prompt (tokens exact, logits within tolerance)
 
-First executed on a B200 in round 2 (green on the first run: profiles/r2_pytest_pending_1gpu.log); part of the default `-m gpu` suite."""
+Part of the default `-m gpu` suite."""
 import types
 
 import numpy as np
@@ -89,7 +89,7 @@ def _paged_prefill_run(q, kc, vc, bt, sids, starts, chunk, prefix, scale, layer)
 def test_prefill_attention_paged_vs_exact_oracle(dtype, geom, prefill_gen):
     nq, nkv, D, bs = geom["nq"], geom["nkv"], geom["D"], geom["bs"]
     if (D == 64 or bs != 16) and prefill_gen.startswith("gen2"):
-        pytest.skip("the tcgen05 kernel serves head_dim 128 / block_size 16; other shapes run gen 1")
+        pytest.skip("the wgmma kernel serves head_dim 128 / block_size 16; other shapes run gen 1")
     L, layer = 2, 1
     #          no prefix | mid-page prefix | page-aligned | 1-token chunk deep in a sequence | chunk > 256 rows (several CTAs) | tiny
     prefix = [0,   13,  64, 500, 100, 3, 255, 0]
@@ -183,7 +183,7 @@ def test_prefill_attention_paged_sarathi_shape_property(prefill_gen):
 # ----------------------------------------------------------------------------- model level
 CFG = dict(model_type="llama", num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, hidden_size=512,
            vocab_size=320, max_position_embeddings=1024, intermediate_size=768, rope_theta=10000.0, rms_norm_eps=1e-5,
-           hidden_act="silu")          # head_dim 128: the tcgen05 kernels serve it
+           hidden_act="silu")          # head_dim 128: the wgmma kernels serve it
 ENG = dict(block_size=16, num_blocks=96, num_cpu_blocks=2, max_seqs_in_block_table=8, max_blocks_per_seq=48)
 
 

@@ -1,7 +1,7 @@
 """GPU: decode-step fusion - rotary embedding + KV store of the new rows in one launch (sllm_rotary_store_kvcache_decode,
 csrc/rotary_store.cu; EngineConfig.fuse_rotary_store) against the two separate kernels (bit for bit) and the oracle.
 
-First executed on a B200 in round 2 (green on the first run: profiles/r2_pytest_pending_1gpu.log); part of the default `-m gpu` suite."""
+Part of the default `-m gpu` suite."""
 import numpy as np
 import pytest
 import torch

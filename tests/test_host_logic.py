@@ -88,24 +88,18 @@ def test_bench_line_contract_helpers():
     assert bench.METRIC == "decode_tokens_per_s" and bench.UNIT == "tokens/s"
 
 
-def test_model_config_matches_the_reference_parser_when_the_reference_is_mounted():
-    """Build-container only (skipped elsewhere): the unmodified reference's LlamaModelConfig and ours expose the same values for
-    every attribute the reference defines, over GQA / MHA / scaled-RoPE / legacy-key configs."""
-    import importlib.util
+def test_model_config_matches_the_reference_parser():
+    """The unmodified reference's LlamaModelConfig and ours expose the same values for every attribute the reference defines,
+    over GQA / MHA / scaled-RoPE / legacy-key configs (reference values recorded in tests/golden/model_config.json by
+    oracle/gen_golden.py)."""
+    import json
     import os
-    import pytest
-    path = "/root/reference/swiftllm/model_config.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not mounted")
-    spec = importlib.util.spec_from_file_location("ref_model_config", path)
-    ref = importlib.util.module_from_spec(spec); spec.loader.exec_module(ref)
-    base = dict(LLAMA3_8B)
-    cfgs = [base, dict(base, rope_scaling={"factor": 8.0, "low_freq_factor": 1.0}),
-            {k: v for k, v in base.items() if k not in ("num_key_value_heads", "rope_theta", "rope_scaling")},
-            dict({k: v for k, v in base.items() if k != "rope_theta"}, rotary_base=12345), dict(base, rope_scaling=2.0)]
-    for c in cfgs:
-        ours, theirs = LlamaModelConfig(c), ref.LlamaModelConfig(c)
-        for name, value in vars(theirs).items():
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "model_config.json")
+    cases = json.load(open(path))["cases"]
+    assert len(cases) == 5
+    for case in cases:
+        ours = LlamaModelConfig(case["config"])
+        for name, value in case["attrs"].items():
             assert getattr(ours, name) == value, name
         for dt in (torch.float16, torch.bfloat16):
-            assert ours.get_kvslot_size(dt) == theirs.get_kvslot_size(dt)
+            assert ours.get_kvslot_size(dt) == case["kvslot_size"][str(dt).split(".")[1]]

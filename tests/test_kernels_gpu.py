@@ -428,7 +428,7 @@ def test_prefill_attention_vs_exact_oracle(dtype, geom, prefill_gen):
 
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_prefill_attention_growing_scores_force_rescales(dtype, prefill_gen):
-    """Adversarial for the lazy-rescale path of the tcgen05 kernel: key magnitudes grow along the sequence and differ
+    """Adversarial for the lazy-rescale path of the wgmma kernel: key magnitudes grow along the sequence and differ
     per row parity, so the running max of SOME rows of a warp jumps by more than 2^8 at several kv steps while their
     neighbours' does not (a per-thread decision around warp-collective TMEM loads/stores must not diverge)."""
     nq, nkv, D = 4, 2, 128

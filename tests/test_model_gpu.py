@@ -4,6 +4,7 @@
  * vs the CPU oracle in bf16; CUDA-graph decode path == eager path."""
 import json
 import os
+import tempfile
 
 import numpy as np
 import pytest
@@ -13,7 +14,8 @@ from oracle.model import OracleLlama, OracleWeights
 
 pytestmark = pytest.mark.gpu
 T = torch.from_numpy
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+# per-step parity numbers of the golden-trace test, appended as JSON lines (outside the source tree)
+OUT = os.environ.get("SLLM_PARITY_LOG_DIR", tempfile.gettempdir())
 
 
 def _hf_tensors(w: OracleWeights, F: int):
@@ -142,7 +144,7 @@ def test_model_vs_cpu_oracle(dtype):
     top-1 margin is clear of the tolerance, logits within 2^-5 (bf16) / 4e-3 (fp16) of max|logit|.  Every
     intermediate activation is rounded to the storage dtype (2^-9 / 2^-12 relative per op) on both sides but GEMM
     accumulation order differs (cuBLAS vs CPU), so ~20 roundings random-walk to a few storage-dtype ulps of the
-    largest logit (observed on B200: 1.6e-2 bf16, 2.2e-3 fp16)."""
+    largest logit (bf16 storage rounding alone is of order 1e-2)."""
     tdt = dict(bfloat16=torch.bfloat16, float16=torch.float16)[dtype]
     w = OracleWeights.random(TINY2, dtype=tdt, seed=3, std=0.05)
     oracle = OracleLlama(TINY2, w, block_size=16, num_blocks=40, num_cpu_blocks=4, max_seqs_in_block_table=16,

@@ -1,7 +1,7 @@
 """GPU: swap with device-resident id lists (sllm_swap_blocks_gathered, csrc/swap_gather.cu; EngineConfig.device_swap) against the
 oracle and the memcpy path (swiftllm_c.swap_blocks): exact bytes, K and V, scattered and consecutive ids, both directions.
 
-First executed on a B200 in round 2 (green on the first run: profiles/r2_pytest_pending_1gpu.log); part of the default `-m gpu` suite."""
+Part of the default `-m gpu` suite."""
 import numpy as np
 import pytest
 import torch

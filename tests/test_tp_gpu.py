@@ -170,12 +170,8 @@ def test_tp_ll_push_exchange_matches_single_gpu(world):
 def test_tp_world8_matches_single_gpu():
     """World 8 (1 kv head / 2 q heads per rank; 3-row decode steps leave five ranks without a row to own): the library default for
     TP 8 (two-shot exchange with in-switch reduction + sharded lm_head + fused rotary / store), the NCCL path and the P2P two-shot
-    kernel against TP = 1, in ONE process group (an 8-GPU box is charged 8x).  SLLM_TP8_MODES=<comma list | all> selects others.
-
-    History: the first version of this test ran all eleven modes (22 tensor-parallel models, ~80 symmetric-memory buffers with
-    multicast bindings) in one process group and did not finish within 400 s on the 8-GPU box of round 2, while every mode takes
-    2-4 s at world 4 (profiles/r2_pytest_tp_n4*.log) and the 8-GPU sweeps of the same kernels ran cleanly
-    (profiles/r2_tp_sweep_n8_b256.jsonl) - which mode stalled is unknown (no per-mode progress lines then; they exist now)."""
+    kernel against TP = 1, in ONE process group.  SLLM_TP8_MODES=<comma list | all> selects others (all eleven modes in one
+    process group means 22 tensor-parallel models and ~80 symmetric-memory buffers with multicast bindings)."""
     if torch.cuda.device_count() < 8:
         pytest.skip("needs 8 GPUs")
     want = os.environ.get("SLLM_TP8_MODES", "default,nccl,fused-two-shot")
