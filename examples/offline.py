@@ -7,6 +7,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     python examples/offline.py --synthetic llama3-8b                     # seeded random weights, random token ids
     ... --chunk 512        prefill the prompts in 512-token chunks through the paged cache (prefill_prefix_lens_list)
     ... --cuda-graph       replay decode steps from CUDA graphs
+    ... --temperature 0.8 --top-p 0.95 [--top-k 50] [--seed 1]    sample instead of greedy decoding
 """
 import argparse
 import os
@@ -20,10 +21,12 @@ import torch  # noqa: E402
 import swiftllm_b200  # noqa: E402
 
 
-def generate(model, input_ids, new_tokens: int, chunk: int = 0):
-    """Greedy generation for a batch of prompts (sequence i uses block-table row i).  chunk > 0: the prompts are prefilled
-    `chunk` tokens at a time through the paged cache.  Returns (token lists, prefill seconds, decode seconds)."""
+def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None):
+    """Generation for a batch of prompts (sequence i uses block-table row i), greedy unless `params` (one
+    swiftllm_b200.SamplingParams for every sequence) is given.  chunk > 0: the prompts are prefilled `chunk` tokens at a time
+    through the paged cache.  Returns (token lists, prefill seconds, decode seconds)."""
     seq_ids = list(range(len(input_ids)))
+    sp = (lambda n: None) if params is None else (lambda n: [params] * n)
     t0 = time.perf_counter()
     if chunk > 0:                      # every call carries the next chunk of each unfinished prompt
         done = [0] * len(input_ids)
@@ -31,20 +34,20 @@ def generate(model, input_ids, new_tokens: int, chunk: int = 0):
         while any(d < len(p) for d, p in zip(done, input_ids)):
             live = [i for i in seq_ids if done[i] < len(input_ids[i])]
             toks = model.forward([input_ids[i][done[i]:done[i] + chunk] for i in live], live, [],
-                                 prefill_prefix_lens_list=[done[i] for i in live])
+                                 prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(len(live)))
             for i, t in zip(live, toks):
                 done[i] = min(len(input_ids[i]), done[i] + chunk)
                 if done[i] == len(input_ids[i]):
                     last[i] = t             # the token sampled after the LAST chunk is the first generated token
     else:
-        last = model.forward(input_ids, seq_ids, [])
+        last = model.forward(input_ids, seq_ids, [], sampling_params_list=sp(len(seq_ids)))
     t_prefill = time.perf_counter() - t0
     outputs = [[t] for t in last]
     seq_lens = [len(p) for p in input_ids]
     t0 = time.perf_counter()
     for _ in range(new_tokens - 1):
         seq_lens = [n + 1 for n in seq_lens]
-        last = model.forward([[t] for t in last], seq_ids, seq_lens)
+        last = model.forward([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(len(seq_ids)))
         for o, t in zip(outputs, last):
             o.append(t)
     return outputs, t_prefill, time.perf_counter() - t0
@@ -59,6 +62,10 @@ def main():
     ap.add_argument("--new-tokens", type=int, default=20)
     ap.add_argument("--chunk", type=int, default=0, help="chunked prefill: tokens of each prompt per forward call (0 = whole prompts)")
     ap.add_argument("--cuda-graph", action="store_true")
+    ap.add_argument("--temperature", type=float, default=0.0, help="0 = greedy decoding")
+    ap.add_argument("--top-k", type=int, default=0, help="keep the k most likely tokens (0 = off)")
+    ap.add_argument("--top-p", type=float, default=1.0, help="keep the smallest set of tokens with this much mass (1 = off)")
+    ap.add_argument("--seed", type=int, default=None, help="sampling seed (default: a fresh one per step from the engine's generator)")
     args = ap.parse_args()
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
@@ -87,7 +94,9 @@ def main():
     model.init_kvcache_and_swap(num_blocks)
     print(f"{num_blocks} KV blocks; model ready in {time.perf_counter() - t0:.1f} s")
 
-    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk)
+    params = None if args.temperature == 0 else \
+        swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed)
+    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params)
     seq_ids = list(range(len(input_ids)))
     for p, o in zip(input_ids, outputs):
         print(f"[{len(p)} prompt tokens] -> {show(o)}")

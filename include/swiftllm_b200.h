@@ -215,6 +215,21 @@ int sllm_swap_blocks_gathered(const int64_t* src_ids, const int64_t* dst_ids, in
                               void* v_cache, void* host_k_swap, void* host_v_swap, int64_t block_bytes,
                               sllm_stream_t stream);
 
+/* ---- Token sampling (new; the reference decodes greedily only, swiftllm/worker/layers/post_layer.py:39):
+ * logits [num_rows, logits_row_stride] 16-bit, the first vocab_size columns of row i are the vocabulary entries
+ * vocab_offset .. vocab_offset + vocab_size - 1 (a vocabulary shard under tensor parallelism, else vocab_offset 0).
+ * Per-row DEVICE arrays [num_rows]: temperature (<= 0: greedy, == torch.argmax), top_k (<= 0 or >= vocab_size: off), top_p
+ * (>= 1: off), seed, pos (the sequence length after this step's input; the noise counter).  Ties at the top-k / top-p boundary
+ * are kept.  out_tokens int64 [num_rows]: GLOBAL token ids.  out_pairs fp32 [num_rows, 2] or NULL: (best score, global index),
+ * the score being the logit for greedy rows and logit / T + Gumbel noise otherwise; the pairs of vocabulary shards merge into
+ * the unsharded result for rows without top-k / top-p (largest score, then smallest index).  Deterministic; a row's token
+ * depends on its logits and parameters only.  Rejected before launch: unknown dtype, vocab_size <= 0 or larger than 8
+ * shared-memory slices (about 819k entries), global indices >= 2^24, a row stride below vocab_size, null pointers. */
+int sllm_sample_tokens(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                       int64_t vocab_offset, const float* temperature, const int32_t* top_k, const float* top_p,
+                       const int64_t* seed, const int32_t* pos, int64_t* out_tokens, float* out_pairs, sllm_dtype_t dtype,
+                       sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

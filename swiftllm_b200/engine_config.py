@@ -52,6 +52,9 @@ class EngineConfig:
     # access.  (The wait cannot be later: freed blocks are handed out again lowest-id-first - the reference's order, which the
     # block-index parity depends on - so the next step's KV store may target exactly the blocks being copied out.)
     swap_on_copy_stream: bool = False
+    # seeds the generator that gives SamplingParams(seed=None) rows a fresh seed each step: runs are reproducible, repeated
+    # prompts still vary
+    sampling_seed: int = 0
 
     @staticmethod
     def add_cli_args(parser: argparse.ArgumentParser):

@@ -1,0 +1,54 @@
+"""Per-request sampling parameters (new: the reference decodes greedily only)."""
+import dataclasses
+import math
+from typing import Optional
+
+import numpy as np
+
+
+@dataclasses.dataclass
+class SamplingParams:
+    """temperature 0 is greedy decoding (top_k / top_p ignored).  top_k 0 and top_p 1 switch those filters off; tokens tied
+    with the last one kept by either filter are kept too.  seed None draws a fresh seed from the model's generator
+    (EngineConfig.sampling_seed), so runs are reproducible while repeated prompts still vary; a fixed seed makes the token a
+    function of the logits, the parameters and the sequence length only."""
+    temperature: float = 0.0
+    top_k: int = 0
+    top_p: float = 1.0
+    seed: Optional[int] = None
+
+    def validate(self):
+        if not (isinstance(self.temperature, (int, float)) and math.isfinite(self.temperature) and self.temperature >= 0):
+            raise ValueError(f"temperature must be a finite number >= 0, got {self.temperature!r}")
+        if isinstance(self.top_k, bool) or not isinstance(self.top_k, (int, np.integer)) or not 0 <= self.top_k < 2 ** 31:
+            raise ValueError(f"top_k must be an integer in [0, 2^31), got {self.top_k!r}")
+        if not (isinstance(self.top_p, (int, float)) and 0 < self.top_p <= 1):
+            raise ValueError(f"top_p must be in (0, 1], got {self.top_p!r}")
+        if self.seed is not None and (isinstance(self.seed, bool) or not isinstance(self.seed, (int, np.integer))
+                                      or not 0 <= self.seed < 2 ** 64):
+            raise ValueError(f"seed must be None or an integer in [0, 2^64), got {self.seed!r}")
+
+
+def _i32(words: np.ndarray) -> list:
+    return words.astype(np.uint32).view(np.int32).tolist()
+
+
+def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator):
+    """Validates the list and returns the staged int32 words (seed lo/hi interleaved [2B], temperature bits [B], top_k [B],
+    top_p bits [B]) and whether any row filters (top-k / top-p); None when every row is greedy.  Raises ValueError."""
+    if len(params_list) != batch_size:
+        raise ValueError(f"sampling_params_list has {len(params_list)} entries for a batch of {batch_size}")
+    for sp in params_list:
+        if not isinstance(sp, SamplingParams):
+            raise ValueError(f"sampling_params_list entries must be SamplingParams, got {type(sp).__name__}")
+        sp.validate()
+    # a fresh seed for every unseeded row, drawn even for greedy rows so the stream does not depend on the batch's mix
+    seeds = np.array([int(rng.integers(0, 2 ** 63)) if sp.seed is None else int(sp.seed) for sp in params_list], dtype=np.uint64)
+    if all(sp.temperature == 0 for sp in params_list):
+        return None
+    temp = np.array([sp.temperature for sp in params_list], dtype=np.float32)
+    top_p = np.array([sp.top_p for sp in params_list], dtype=np.float32)
+    top_k = [int(sp.top_k) for sp in params_list]
+    filtered = any(sp.temperature > 0 and (sp.top_k > 0 or sp.top_p < 1) for sp in params_list)
+    words = _i32(seeds.view(np.uint32)) + _i32(temp.view(np.uint32)) + top_k + _i32(top_p.view(np.uint32))
+    return words, filtered

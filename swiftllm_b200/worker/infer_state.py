@@ -49,3 +49,23 @@ class LlamaInferState:
     # the KV cache.  None = whole prompts, attention over the packed k/v.
     prefill_prefix_lens: Optional[torch.Tensor] = None  # [num_prefill_seqs]
     max_prefill_kv_len: int = 0                          # max_i(prefix_i + chunk_i); 0 when not chunked
+    # Per-row sampling parameters (SamplingParams) on the device; None = greedy argmax for every row
+    sampling: Optional["SamplingState"] = None
+
+
+@dataclasses.dataclass
+class SamplingState:
+    temperature: torch.Tensor       # [batch_size] float32, 0 = greedy row
+    top_k: torch.Tensor             # [batch_size] int32
+    top_p: torch.Tensor             # [batch_size] float32
+    seed: torch.Tensor              # [batch_size] int64
+    pos: torch.Tensor               # [batch_size] int32: sequence length after this step's input (noise counter)
+    filtered: bool                  # some row uses top-k or top-p (needs the whole vocabulary row on one rank)
+
+    @staticmethod
+    def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool) -> "SamplingState":
+        """`words`: the int32 device view staged from swiftllm_b200.sampling_params.sampling_words (8-byte aligned)."""
+        B = pos.shape[0]
+        return SamplingState(temperature=words[2 * B:3 * B].view(torch.float32), top_k=words[3 * B:4 * B],
+                             top_p=words[4 * B:5 * B].view(torch.float32), seed=words[:2 * B].view(torch.int64), pos=pos,
+                             filtered=filtered)

@@ -2,13 +2,19 @@
 
 Addition (tensor parallelism, SURVEY.md §8 f-3): with a vocabulary-sharded lm_head every rank computes the logits of its
 V / tp_size rows only and the greedy token is found with ONE all-gather of per-rank (max logit, global index) pairs
-(8 bytes per sequence and rank) instead of every rank streaming the whole lm_head."""
+(8 bytes per sequence and rank) instead of every rank streaming the whole lm_head.
+
+Addition (sampling, csrc/sampling.cu): when the step carries sampling parameters (infer_state.sampling) the token comes from the
+sampling kernel instead of argmax.  With a sharded lm_head, batches without top-k / top-p sample each shard and exchange
+(best score, global index) pairs through the same all-gather - the noise is keyed by the global index, so the merged token is
+the unsharded one; otherwise the logits are all-gathered and every rank samples the full rows."""
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.linear import linear
 from swiftllm_b200.worker.kernels.rmsnorm import rmsnorm_inplace
+from swiftllm_b200.worker.kernels.sampling import sample_tokens
 
 
 def merge_sharded_argmax(pairs: torch.Tensor) -> torch.Tensor:
@@ -44,20 +50,38 @@ class LlamaPostLayer:
         if not already_normed:
             rmsnorm_inplace(last_input, self.weights.final_norm, self.model_config.rms_norm_eps)
         logits = linear(last_input, self.weights.lm_head)      # [batch_size, vocab_size] (or this rank's V / tp_size columns)
+        sp = infer_state.sampling
         if not self.sharded:
             if self.keep_logits:
                 self.last_logits = logits
+            if sp is not None:
+                return sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
             return torch.argmax(logits, dim=1)
 
         B, Vs = logits.shape
-        local = torch.argmax(logits, dim=1)
-        mine = torch.stack((logits.gather(1, local[:, None]).squeeze(1).float(),
-                            (local + self.tp_rank * Vs).float()), dim=1)             # [B, 2]
+        if sp is not None and sp.filtered:                     # top-k / top-p need whole rows: gather them, sample on every rank
+            full = self._gather_logits(logits)
+            if self.keep_logits:
+                self.last_logits = full
+            return sample_tokens(full, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+        if sp is not None:
+            mine = torch.empty((B, 2), dtype=torch.float32, device=logits.device)
+            sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos, vocab_offset=self.tp_rank * Vs,
+                          out_pairs=mine)
+        else:
+            local = torch.argmax(logits, dim=1)
+            mine = torch.stack((logits.gather(1, local[:, None]).squeeze(1).float(),
+                                (local + self.tp_rank * Vs).float()), dim=1)             # [B, 2]
         # outputs in the concatenated form ([ranks * B, ...]): accepted by both NCCL and gloo
         pairs = torch.empty((self.tp_size * B, 2), dtype=torch.float32, device=logits.device)
         dist.all_gather_into_tensor(pairs, mine.contiguous(), group=self.tp_group)
         if self.keep_logits:                                   # parity tests only: reassemble the full logits
-            full = torch.empty((self.tp_size * B, Vs), dtype=logits.dtype, device=logits.device)
-            dist.all_gather_into_tensor(full, logits.contiguous(), group=self.tp_group)
-            self.last_logits = full.view(self.tp_size, B, Vs).permute(1, 0, 2).reshape(B, self.tp_size * Vs)
+            self.last_logits = self._gather_logits(logits)
         return merge_sharded_argmax(pairs.view(self.tp_size, B, 2))
+
+    def _gather_logits(self, logits: torch.Tensor) -> torch.Tensor:
+        """[B, V / tp_size] shards of every rank -> [B, V] (vocabulary order)."""
+        B, Vs = logits.shape
+        full = torch.empty((self.tp_size * B, Vs), dtype=logits.dtype, device=logits.device)
+        dist.all_gather_into_tensor(full, logits.contiguous(), group=self.tp_group)
+        return full.view(self.tp_size, B, Vs).permute(1, 0, 2).reshape(B, self.tp_size * Vs)

@@ -25,11 +25,12 @@ import torch.distributed as dist
 from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
+from swiftllm_b200.sampling_params import sampling_words
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.weight import load_weights
 
-from .infer_state import LlamaInferState
+from .infer_state import LlamaInferState, SamplingState
 from .layers.post_layer import LlamaPostLayer
 from .layers.pre_layer import LlamaPreLayer
 from .layers.transformer_layer import LlamaTransformerLayer
@@ -106,6 +107,8 @@ class LlamaModel:
         self._stage_next = 0
         self._swap_stream = None        # EngineConfig.swap_on_copy_stream: dedicated copy stream + "copies done" event
         self._swap_done = None
+        # seeds of SamplingParams(seed=None) rows: every rank of a tensor-parallel group draws the same sequence
+        self._sampling_rng = np.random.default_rng(getattr(engine_config, "sampling_seed", 0))
 
     # ------------------------------------------------------------------ init
     @torch.inference_mode()
@@ -291,7 +294,8 @@ class LlamaModel:
 
     @torch.inference_mode()
     def forward(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
-                ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None) -> list:
+                ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
+                sampling_params_list: Optional[list] = None) -> list:
         """model.py:252-359.  Batch layout contract: prefill sequences first (full prompt each), then decoding
         sequences (exactly one token each); decoding_seq_lens_list[i] includes the new token.
 
@@ -300,15 +304,22 @@ class LlamaModel:
         prefill_prefix_lens_list[i]; positions below it were written to the KV cache by earlier calls.  The chunk's
         K/V are stored at their positions and its queries attend to the whole prefix + chunk through the block
         table.  The token returned for a prefill entry is sampled after the chunk's last token (meaningful for the
-        final chunk of a prompt only)."""
+        final chunk of a prompt only).
+
+        `sampling_params_list` (addition): one swiftllm_b200.SamplingParams per batch entry; the token of entry i is drawn with
+        its temperature / top-k / top-p and seed (csrc/sampling.cu), the noise keyed by the sequence length after this step.
+        None (or every temperature 0) is greedy decoding, the reference's behaviour.  Invalid parameters raise ValueError
+        before anything is enqueued."""
         return self.forward_async(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache,
-                                  prefill_prefix_lens_list).tolist()
+                                  prefill_prefix_lens_list, sampling_params_list).tolist()
 
     @torch.inference_mode()
     def forward_async(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False,
-                      prefill_prefix_lens_list=None) -> torch.Tensor:
+                      prefill_prefix_lens_list=None, sampling_params_list=None) -> torch.Tensor:
         """Same as forward() but returns the token tensor on the device (no sync)."""
         mc = self.model_config
+        samp = None if sampling_params_list is None else \
+            sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         num_prefill_seqs = len(input_ids_list) - len(decoding_seq_lens_list)
         flat_ids = list(itertools.chain(*input_ids_list))
         prefill_lens = [len(s) for s in input_ids_list[:num_prefill_seqs]]
@@ -335,11 +346,14 @@ class LlamaModel:
 
         if (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
                 and batch_size > 0):
-            return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len)
+            return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp)
 
-        ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = self._stage_metadata(
-            flat_ids, seq_ids_list, seq_lengths_list, prefill_lens, prefill_starts, positions, last_idx,
-            prefix_lens if chunked else [])
+        # the sampling words go first: the int64 seeds need an 8-byte aligned offset
+        views = self._stage_metadata(
+            *([samp[0]] if samp else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens, prefill_starts, positions,
+            last_idx, prefix_lens if chunked else [])
+        ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = views[-8:]
+        sampling = SamplingState.from_staged(views[0], seq_lengths, samp[1]) if samp else None
 
         if not ignore_kvcache:
             self.gpu_block_manager.allocate_blocks_for_seqs(seq_ids, seq_lengths, seq_ids_list=seq_ids_list,
@@ -364,14 +378,16 @@ class LlamaModel:
             paged_attn_seq_block_size=0, last_token_indices=last,
             prefill_prefix_lens=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0,
+            sampling=sampling,
         )
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
-    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len):
+    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None):
         """Pure-decode step replayed from a CUDA graph.  Static device buffers hold the step's metadata; the graph
         (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
-        allocation, gathers, every layer, lm_head and argmax."""
+        allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
+        filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy."""
         from swiftllm_b200 import _lib
         B = len(flat_ids)
         mc = self.model_config
@@ -381,6 +397,9 @@ class LlamaModel:
         bucket = ((max_len + 1023) // 1024) * 1024
         ws_bytes = _lib.lib().sllm_paged_attention_workspace_bytes(B, nq, mc.head_dim, bucket, 0, nkv)
         key = (B, bucket if ws_bytes > 0 else 0)
+        if samp:
+            # sharded lm_head: filtered rows sample the gathered full rows, the others exchange per-shard pairs
+            key += (True, samp[1] and self.post_layer.sharded)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -388,7 +407,7 @@ class LlamaModel:
             cap = max(1, int(getattr(self.engine_config, "max_cuda_graphs", 16)))
             while len(self._graphs) >= cap:
                 self._graphs.pop(next(iter(self._graphs)))
-            g = self._capture_decode_graph(B, bucket)
+            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1])
         self._graphs[key] = g                    # (re)insert as most recently used
         # host-side bookkeeping of the allocator (exhaustion check + mirror), no device work here
         bm = self.gpu_block_manager
@@ -408,6 +427,9 @@ class LlamaModel:
         host, ev = g["host"][i]
         ev.synchronize()
         hv = host.numpy()
+        if samp:
+            hv[:5 * B] = samp[0]
+            hv = hv[5 * B:]
         hv[:B] = flat_ids; hv[B:2 * B] = seq_ids_list; hv[2 * B:3 * B] = lens_list
         g["meta"].copy_(host, non_blocking=True)
         ev.record()
@@ -416,13 +438,16 @@ class LlamaModel:
         # the graph's static output is overwritten by the next replay: hand out a copy (stream-ordered, no sync)
         return g["tokens"].clone()
 
-    def _capture_decode_graph(self, B: int, bucket_len: int):
+    def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None):
+        """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words."""
         from swiftllm_b200.worker.kernels.block_mgmt import allocate_blocks_for_seqs as alloc_kernel
         mc, ec = self.model_config, self.engine_config
         dev = self.device
-        meta = torch.zeros((3 * B,), dtype=torch.int32, device=dev)
-        host = [(torch.zeros((3 * B,), dtype=torch.int32).pin_memory(), torch.cuda.Event()) for _ in range(self._STAGE_SLOTS)]
-        ids, seq_ids, lens = meta[:B], meta[B:2 * B], meta[2 * B:]
+        nw = 0 if filtered is None else 5 * B
+        meta = torch.zeros((nw + 3 * B,), dtype=torch.int32, device=dev)
+        host = [(torch.zeros((nw + 3 * B,), dtype=torch.int32).pin_memory(), torch.cuda.Event()) for _ in range(self._STAGE_SLOTS)]
+        ids, seq_ids, lens = meta[nw:nw + B], meta[nw + B:nw + 2 * B], meta[nw + 2 * B:]
+        sampling = None if filtered is None else SamplingState.from_staged(meta[:nw], lens, filtered)
         last = torch.arange(B, dtype=torch.int32, device=dev)
         empty = torch.empty((0,), dtype=torch.int32, device=dev)
 
@@ -437,7 +462,7 @@ class LlamaModel:
                 num_decoding_seqs=B, decoding_seq_lens=lens, max_decoding_len=bucket_len,
                 seq_block_size=2048, num_seq_blocks=(bucket_len + 2047) // 2048,
                 position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last)
+                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=sampling)
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
