@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+from attention_check import check_attention
 from oracle import kernels as K
 
 pytestmark = pytest.mark.gpu
@@ -296,7 +297,7 @@ def _gz(z, c):
 def test_paged_attention_golden(golden, case, sbs, paged_gen):
     """vs the reference's own outputs.  The reference accumulates q.k in fp16 (its own error vs fp64 is 1-3e-3 of
     max|o|, SURVEY.md §7); this kernel accumulates in fp32, so the tolerance is 3e-3 * max|o| against the reference
-    and 1e-3 * max|o| against the fp64 definition."""
+    and 1e-3 * max|o| against the fp64 definition (plus the per-(sequence, head) check of tests/attention_check.py)."""
     z = golden("paged_attention")
     args = _gz(z, case)
     s = int(z[f"{case}_seq_block_size"]) if sbs == "ref" else 0
@@ -305,6 +306,7 @@ def test_paged_attention_golden(golden, case, sbs, paged_gen):
     o64 = K.paged_attention_exact(*args)
     assert (o.double() - o_ref.double()).abs().max() <= 3e-3 * o64.abs().max()
     assert (o.double() - o64).abs().max() <= 1e-3 * o64.abs().max()
+    check_attention(o, o64, args[0].shape[1], args[5], what="decode")
 
 
 @pytest.fixture(params=["gen2-tcgen05", "gen1-mma.sync"])
@@ -316,8 +318,12 @@ def paged_gen(request, monkeypatch):
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
+# GQA groups 1, 4, 8, 16 and the groups of real models that are not powers of two: 3 (24/8 heads, and head_dim 64),
+# 5 (40/8), 6 (12/2), 7 (28/4), 12 (24/2); the wgmma kernel pads them to 8 or 16 heads
 @pytest.mark.parametrize("geom", [dict(nq=4, nkv=4, D=64), dict(nq=8, nkv=2, D=128), dict(nq=32, nkv=8, D=128),
-                                  dict(nq=8, nkv=1, D=128), dict(nq=16, nkv=1, D=128), dict(nq=4, nkv=4, D=128)])
+                                  dict(nq=8, nkv=1, D=128), dict(nq=16, nkv=1, D=128), dict(nq=4, nkv=4, D=128),
+                                  dict(nq=12, nkv=4, D=64), dict(nq=24, nkv=8, D=128), dict(nq=40, nkv=8, D=128),
+                                  dict(nq=12, nkv=2, D=128), dict(nq=28, nkv=4, D=128), dict(nq=24, nkv=2, D=128)])
 @pytest.mark.parametrize("sbs", [0, 64, 256])
 def test_paged_attention_vs_exact_oracle(dtype, geom, sbs, paged_gen):
     nq, nkv, D = geom["nq"], geom["nkv"], geom["D"]
@@ -340,8 +346,7 @@ def test_paged_attention_vs_exact_oracle(dtype, geom, sbs, paged_gen):
     scale = D ** -0.5
     o64 = K.paged_attention_exact(q, kc, vc, bt, sids, lens, scale, bs, 1)
     o = _paged_run(q, kc, vc, bt, sids, lens, scale, bs, 1, sbs=sbs)
-    tol = 1.5e-3 if dtype == torch.float16 else 8e-3        # output rounding (2^-11 / 2^-8) + P rounding before P.V
-    assert (o.double() - o64).abs().max() <= tol * o64.abs().max()
+    check_attention(o, o64, nq, lens, what="decode")
 
 
 def test_paged_attention_full_length_properties(paged_gen):
@@ -365,7 +370,7 @@ def test_paged_attention_full_length_properties(paged_gen):
     scale = D ** -0.5
     o1 = _paged_run(q, kc, vc, table(ident), sids, lens, scale, bs, 0)
     o64 = K.paged_attention_exact(q, kc, vc, table(ident), sids, lens, scale, bs, 0)
-    assert (o1.double() - o64).abs().max() <= 8e-3 * o64.abs().max()
+    check_attention(o1, o64, nq, lens, what="decode")
     o2 = _paged_run(q, kc, vc, table(ident), sids, lens, scale, bs, 0, sbs=512)          # forced flash-decoding split
     assert (o1.float() - o2.float()).abs().max() <= 2 ** -7 * o64.abs().max()           # both round to bf16 once
     perm = torch.randperm(nblk, generator=g).tolist()
@@ -404,11 +409,13 @@ def test_prefill_attention_golden(golden, prefill_gen):
     o = _prefill_run(q, k, v, z["start_locs"], z["seq_lens"], float(z["scale"]))
     o64 = K.prefill_attention_exact(q, k, v, z["start_locs"], z["seq_lens"], float(z["scale"]))
     assert (o.double() - T(z["o"]).double()).abs().max() <= 2e-3 * o64.abs().max()
-    assert (o.double() - o64).abs().max() <= 1.5e-3 * o64.abs().max()
+    check_attention(o, o64, q.shape[1], z["seq_lens"], starts=z["start_locs"], what="prefill")
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("geom", [dict(nq=4, nkv=2, D=64), dict(nq=8, nkv=2, D=128), dict(nq=4, nkv=4, D=128)])
+@pytest.mark.parametrize("geom", [dict(nq=4, nkv=2, D=64), dict(nq=8, nkv=2, D=128), dict(nq=4, nkv=4, D=128),
+                                  dict(nq=12, nkv=4, D=64), dict(nq=24, nkv=8, D=128), dict(nq=40, nkv=8, D=128),
+                                  dict(nq=12, nkv=2, D=128), dict(nq=28, nkv=4, D=128), dict(nq=24, nkv=2, D=128)])
 def test_prefill_attention_vs_exact_oracle(dtype, geom, prefill_gen):
     nq, nkv, D = geom["nq"], geom["nkv"], geom["D"]
     if D == 64 and prefill_gen.startswith("gen2"):
@@ -421,8 +428,7 @@ def test_prefill_attention_vs_exact_oracle(dtype, geom, prefill_gen):
     v = torch.randn(Tn, nkv, D, generator=g).to(dtype)
     o = _prefill_run(q, k, v, starts, lens, D ** -0.5)
     o64 = K.prefill_attention_exact(q, k, v, starts, lens, D ** -0.5)
-    tol = 1.5e-3 if dtype == torch.float16 else 8e-3
-    assert (o.double() - o64).abs().max() <= tol * o64.abs().max()
+    check_attention(o, o64, nq, lens, starts=starts, what="prefill")
     assert (o[sum(lens):] == 0).all()
 
 
@@ -446,9 +452,8 @@ def test_prefill_attention_growing_scores_force_rescales(dtype, prefill_gen):
     q, k, v = q.to(dtype), k.to(dtype), v.to(dtype)
     o = _prefill_run(q, k, v, starts, lens, D ** -0.5)
     o64 = K.prefill_attention_exact(q, k, v, starts, lens, D ** -0.5)
-    tol = 2e-3 if dtype == torch.float16 else 1e-2
     assert torch.isfinite(o.float()).all()
-    assert (o.double() - o64).abs().max() <= tol * o64.abs().max()
+    check_attention(o, o64, nq, lens, starts=starts, tol=2e-3 if dtype == torch.float16 else 1e-2, what="prefill")
 
 
 def test_prefill_attention_long_sequence_property(prefill_gen):
@@ -465,24 +470,29 @@ def test_prefill_attention_long_sequence_property(prefill_gen):
     bt = torch.arange(Ln // bs, dtype=torch.int32).unsqueeze(0)
     od = _paged_run(q[-1:].contiguous(), kc, vc, bt, [0], [Ln], D ** -0.5, bs, 0)
     ref = K.paged_attention_exact(q[-1:], kc, vc, bt, [0], [Ln], D ** -0.5, bs, 0)
-    assert (o[-1].reshape(-1).double() - ref[0]).abs().max() <= 8e-3 * ref.abs().max()
-    assert (od[0].double() - ref[0]).abs().max() <= 8e-3 * ref.abs().max()
+    check_attention(o[-1], ref[0], nq, [Ln], what="prefill")
+    check_attention(od, ref, nq, [Ln], what="decode")
     # spot-check a few earlier rows against the fp64 definition
     for r in (0, 1, 127, 128, 2047, 3000):
         rr = K.paged_attention_exact(q[r:r + 1], kc, vc, bt, [0], [r + 1], D ** -0.5, bs, 0)
-        assert (o[r].reshape(-1).double() - rr[0]).abs().max() <= 8e-3 * max(rr.abs().max(), 1e-3)
+        check_attention(o[r], rr[0], nq, [r + 1], what="prefill")
 
 
 # ----------------------------------------------------------------------------- row-strided q/k/v (fused QKV GEMM output)
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_kernels_accept_fused_qkv_column_slices(dtype, paged_gen, prefill_gen):
+    check_fused_qkv_column_slices(dtype, 8, 2)
+
+
+def check_fused_qkv_column_slices(dtype, nq, nkv):
     """q, k, v as column slices of one [T, (nq + 2 nkv) D] buffer (what the fused QKV GEMM produces) must give exactly
-    the results of separate contiguous tensors: rotary, KV store, prefill attention, paged attention."""
+    the results of separate contiguous tensors: rotary, KV store, prefill attention, chunked prefill attention, paged
+    attention; the attention outputs also match the fp64 definition."""
     from swiftllm_b200.worker.kernels.rotary_emb import rotary_embedding_inplace
     from swiftllm_b200.worker.kernels.kvcache_mgmt import store_kvcache
-    from swiftllm_b200.worker.kernels.prefill_attn import prefill_attention
+    from swiftllm_b200.worker.kernels.prefill_attn import prefill_attention, prefill_attention_paged
     from swiftllm_b200.worker.kernels.paged_attn import paged_attention
-    nq, nkv, D, bs, L = 8, 2, 128, 16, 2
+    D, bs, L = 128, 16, 2
     plens, dlens = [130, 17], [300, 45, 64]
     Tp, Bd = sum(plens), len(dlens)
     Tn = Tp + Bd
@@ -516,9 +526,27 @@ def test_kernels_accept_fused_qkv_column_slices(dtype, paged_gen, prefill_gen):
     o1 = torch.zeros(Tp, nq, D, dtype=dtype, device=DEV); o2 = torch.zeros_like(o1)
     prefill_attention(qs[:Tp], ks[:Tp], vs[:Tp], o1, None, None, st); prefill_attention(qc[:Tp].contiguous(), kc_[:Tp].contiguous(), vc_[:Tp].contiguous(), o2, None, None, st)
     assert torch.equal(o1, o2)
+    starts = [0, plens[0]]
+    ref = K.prefill_attention_exact(qc[:Tp].cpu(), kc_[:Tp].cpu(), vc_[:Tp].cpu(), starts, plens, D ** -0.5)
+    check_attention(o1, ref, nq, plens, starts=starts, what="prefill")
+    # chunked prefill over the cache just written: the prompts' last 40 / 9 tokens as chunks after their prefixes
+    chunk, prefix = [40, 9], [plens[0] - 40, plens[1] - 9]
+    qpk = torch.cat([qc[prefix[0]:plens[0]], qc[plens[0] + prefix[1]:Tp]])
+    stc = NS(num_prefill_seqs=2, seq_ids=st.seq_ids, prefill_seq_start_locs=i32([0, chunk[0]]), prefill_seq_lens=i32(chunk),
+             prefill_prefix_lens=i32(prefix), max_prefill_len=max(chunk), softmax_scale=D ** -0.5)
+    qbuf = torch.zeros(sum(chunk), (nq + 2 * nkv) * D, dtype=dtype, device=DEV)
+    qbuf[:, : nq * D] = qpk.flatten(1)
+    qstr = qbuf[:, : nq * D].unflatten(1, (nq, D))                                                  # row stride (nq + 2 nkv) D
+    p1 = torch.zeros(sum(chunk), nq, D, dtype=dtype, device=DEV); p2 = torch.zeros_like(p1)
+    prefill_attention_paged(qstr, k1, v1, bt, p1, None, None, stc, 1)
+    prefill_attention_paged(qpk.contiguous(), k1, v1, bt, p2, None, None, stc, 1)
+    assert torch.equal(p1, p2)
+    ref = K.prefix_prefill_attention_exact(qpk.cpu(), k1.cpu(), v1.cpu(), bt.cpu().numpy(), [0, 1], [0, chunk[0]], chunk, prefix,
+                                           D ** -0.5, bs, 1)
+    check_attention(p1, ref, nq, chunk, starts=[0, chunk[0]], prefix=prefix, what="paged_prefill")
     d1 = torch.zeros(Bd, nq * D, dtype=dtype, device=DEV); d2 = torch.zeros_like(d1)
     paged_attention(qs[Tp:], k1, v1, bt, None, NS(block_size=bs), st, 1, d1)
     paged_attention(qc[Tp:].contiguous(), k1, v1, bt, None, NS(block_size=bs), st, 1, d2)
     assert torch.equal(d1, d2)
     ref = K.paged_attention_exact(qc[Tp:].cpu(), k1.cpu(), v1.cpu(), bt.cpu(), [2, 3, 4], dlens, D ** -0.5, bs, 1)
-    assert (d1.cpu().double() - ref).abs().max() <= (2e-3 if dtype == torch.float16 else 1e-2) * ref.abs().max()
+    check_attention(d1, ref, nq, dlens, tol=2e-3 if dtype == torch.float16 else 1e-2, what="decode")
