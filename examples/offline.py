@@ -8,6 +8,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --chunk 512        prefill the prompts in 512-token chunks through the paged cache (prefill_prefix_lens_list)
     ... --cuda-graph       replay decode steps from CUDA graphs
     ... --temperature 0.8 --top-p 0.95 [--top-k 50] [--seed 1]    sample instead of greedy decoding
+    ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
 """
 import argparse
 import os
@@ -21,33 +22,49 @@ import torch  # noqa: E402
 import swiftllm_b200  # noqa: E402
 
 
-def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None):
+def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None):
     """Generation for a batch of prompts (sequence i uses block-table row i), greedy unless `params` (one
     swiftllm_b200.SamplingParams for every sequence) is given.  chunk > 0: the prompts are prefilled `chunk` tokens at a time
-    through the paged cache.  Returns (token lists, prefill seconds, decode seconds)."""
+    through the paged cache.  Returns (token lists, prefill seconds, decode seconds).
+    With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token."""
     seq_ids = list(range(len(input_ids)))
     sp = (lambda n: None) if params is None else (lambda n: [params] * n)
+    want_lp = params is not None and params.logprobs is not None
+    logs = logs if logs is not None else [[] for _ in input_ids]
+
+    def step(*args, **kw):
+        if not want_lp:
+            return model.forward(*args, **kw)
+        return model.forward_with_logprobs(*args, **kw)
     t0 = time.perf_counter()
     if chunk > 0:                      # every call carries the next chunk of each unfinished prompt
         done = [0] * len(input_ids)
         last = [None] * len(input_ids)
         while any(d < len(p) for d, p in zip(done, input_ids)):
             live = [i for i in seq_ids if done[i] < len(input_ids[i])]
-            toks = model.forward([input_ids[i][done[i]:done[i] + chunk] for i in live], live, [],
-                                 prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(len(live)))
+            toks = step([input_ids[i][done[i]:done[i] + chunk] for i in live], live, [],
+                        prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(len(live)))
             for i, t in zip(live, toks):
                 done[i] = min(len(input_ids[i]), done[i] + chunk)
                 if done[i] == len(input_ids[i]):
                     last[i] = t             # the token sampled after the LAST chunk is the first generated token
     else:
-        last = model.forward(input_ids, seq_ids, [], sampling_params_list=sp(len(seq_ids)))
+        last = step(input_ids, seq_ids, [], sampling_params_list=sp(len(seq_ids)))
+    if want_lp:
+        for lg, r in zip(logs, last):
+            lg.append(r)
+        last = [r.token for r in last]
     t_prefill = time.perf_counter() - t0
     outputs = [[t] for t in last]
     seq_lens = [len(p) for p in input_ids]
     t0 = time.perf_counter()
     for _ in range(new_tokens - 1):
         seq_lens = [n + 1 for n in seq_lens]
-        last = model.forward([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(len(seq_ids)))
+        last = step([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(len(seq_ids)))
+        if want_lp:
+            for lg, r in zip(logs, last):
+                lg.append(r)
+            last = [r.token for r in last]
         for o, t in zip(outputs, last):
             o.append(t)
     return outputs, t_prefill, time.perf_counter() - t0
@@ -66,6 +83,7 @@ def main():
     ap.add_argument("--top-k", type=int, default=0, help="keep the k most likely tokens (0 = off)")
     ap.add_argument("--top-p", type=float, default=1.0, help="keep the smallest set of tokens with this much mass (1 = off)")
     ap.add_argument("--seed", type=int, default=None, help="sampling seed (default: a fresh one per step from the engine's generator)")
+    ap.add_argument("--logprobs", type=int, default=None, help="print each token's log-probability and the N most likely tokens (0..20)")
     args = ap.parse_args()
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
@@ -94,12 +112,16 @@ def main():
     model.init_kvcache_and_swap(num_blocks)
     print(f"{num_blocks} KV blocks; model ready in {time.perf_counter() - t0:.1f} s")
 
-    params = None if args.temperature == 0 else \
-        swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed)
-    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params)
+    params = None if args.temperature == 0 and args.logprobs is None else \
+        swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs)
+    logs = [[] for _ in input_ids]
+    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs)
     seq_ids = list(range(len(input_ids)))
-    for p, o in zip(input_ids, outputs):
+    for p, o, lg in zip(input_ids, outputs, logs):
         print(f"[{len(p)} prompt tokens] -> {show(o)}")
+        for r in lg:      # log-probabilities of the raw model distribution (before temperature / top-k / top-p)
+            top = ", ".join(f"{show([t])!r}:{lp:.3f}" for t, lp in r.top)
+            print(f"    {show([r.token])!r} {r.logprob:.4f}   top [{top}]")
     print(f"prefill {t_prefill * 1e3:.1f} ms ({sum(map(len, input_ids)) / t_prefill:.0f} tok/s), "
           f"decode {t_decode / max(1, args.new_tokens - 1) * 1e3:.2f} ms/step")
     model.free_seqs_resources(seq_ids)

@@ -230,6 +230,20 @@ int sllm_sample_tokens(const void* logits, int64_t num_rows, int vocab_size, int
                        const int64_t* seed, const int32_t* pos, int64_t* out_tokens, float* out_pairs, sllm_dtype_t dtype,
                        sllm_stream_t stream);
 
+/* ---- Token log-probabilities (new; the reference returns token ids only): log_softmax of the raw 16-bit logits (no
+ * temperature, no top-k / top-p), logits as in sllm_sample_tokens with the whole vocabulary in each row.
+ * m = the largest logit, Z = sum_v round(expf(l_v - m) * 2^40) as an exact 64-bit integer, lse = m + logf(Z * 2^-40) and
+ * logprob(v) = l_v - lse, all fp32.  token_ids int64 [num_rows]: out_token_logprob fp32 [num_rows] = logprob(token_ids[i]), NaN
+ * for an id outside [0, vocab_size).  top_n in [0, 20]: out_top_ids int32 / out_top_logprobs fp32 [num_rows, top_n] = the
+ * min(top_n, vocab_size) ids with the largest logits, ordered by (logit desc, id asc), -0 == +0; later entries are id -1, NaN.
+ * A row holding a NaN or +inf (or only -inf) gives NaN logprobs; a -inf logit gives -inf.  Deterministic: a row's outputs
+ * depend on its logits only.  Rejected before launch: unknown dtype, vocab_size <= 0 or larger than 8 shared-memory slices,
+ * top_n outside [0, 20], a row stride below vocab_size, num_rows outside [0, 2^20], null pointers (out_top_* may be NULL
+ * when top_n is 0). */
+int sllm_token_logprobs(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                        const int64_t* token_ids, int top_n, float* out_token_logprob, int32_t* out_top_ids,
+                        float* out_top_logprobs, sllm_dtype_t dtype, sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,9 +1,11 @@
-"""Per-request sampling parameters (new: the reference decodes greedily only)."""
+"""Per-request sampling parameters and log-probability results (new: the reference decodes greedily only)."""
 import dataclasses
 import math
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
+
+MAX_LOGPROBS = 20                   # csrc/logprobs.cu: kMaxTopN
 
 
 @dataclasses.dataclass
@@ -11,11 +13,16 @@ class SamplingParams:
     """temperature 0 is greedy decoding (top_k / top_p ignored).  top_k 0 and top_p 1 switch those filters off; tokens tied
     with the last one kept by either filter are kept too.  seed None draws a fresh seed from the model's generator
     (EngineConfig.sampling_seed), so runs are reproducible while repeated prompts still vary; a fixed seed makes the token a
-    function of the logits, the parameters and the sequence length only."""
+    function of the logits, the parameters and the sequence length only.
+
+    logprobs (LlamaModel.forward_with_logprobs): None returns none, 0 the returned token's log-probability, 1..20 also the
+    top-N alternatives.  They are log_softmax of the raw logits - the model's distribution before temperature, top-k and top-p.
+    forward / forward_async ignore the field."""
     temperature: float = 0.0
     top_k: int = 0
     top_p: float = 1.0
     seed: Optional[int] = None
+    logprobs: Optional[int] = None
 
     def validate(self):
         if not (isinstance(self.temperature, (int, float)) and math.isfinite(self.temperature) and self.temperature >= 0):
@@ -27,6 +34,24 @@ class SamplingParams:
         if self.seed is not None and (isinstance(self.seed, bool) or not isinstance(self.seed, (int, np.integer))
                                       or not 0 <= self.seed < 2 ** 64):
             raise ValueError(f"seed must be None or an integer in [0, 2^64), got {self.seed!r}")
+        if self.logprobs is not None and (isinstance(self.logprobs, bool) or not isinstance(self.logprobs, (int, np.integer))
+                                          or not 0 <= self.logprobs <= MAX_LOGPROBS):
+            raise ValueError(f"logprobs must be None or an integer in [0, {MAX_LOGPROBS}], got {self.logprobs!r}")
+
+
+class TokenLogprobs(NamedTuple):
+    """One batch entry of LlamaModel.forward_with_logprobs.  logprob: log-probability of `token` under the raw model
+    distribution (log_softmax of the logits); top: [(token id, logprob)] of the N most likely tokens, most likely first, ties
+    broken by the smaller id (the empty list for logprobs=0).  Both None when the entry did not ask."""
+    token: int
+    logprob: Optional[float] = None
+    top: Optional[list] = None
+
+
+def logprobs_top_n(params_list: Optional[list]) -> Optional[int]:
+    """The per-launch N: the largest `logprobs` of the (validated) list, None when no entry asks."""
+    asked = [int(sp.logprobs) for sp in params_list or [] if sp.logprobs is not None]
+    return max(asked) if asked else None
 
 
 def _i32(words: np.ndarray) -> list:

@@ -51,6 +51,9 @@ class LlamaInferState:
     max_prefill_kv_len: int = 0                          # max_i(prefix_i + chunk_i); 0 when not chunked
     # Per-row sampling parameters (SamplingParams) on the device; None = greedy argmax for every row
     sampling: Optional["SamplingState"] = None
+    # Top-N of the step's log-probabilities (the largest SamplingParams.logprobs of the batch); None = no log-probabilities,
+    # and the post layer returns the token tensor alone
+    logprobs: Optional[int] = None
 
 
 @dataclasses.dataclass

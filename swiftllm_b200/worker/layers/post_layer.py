@@ -7,12 +7,18 @@ V / tp_size rows only and the greedy token is found with ONE all-gather of per-r
 Addition (sampling, csrc/sampling.cu): when the step carries sampling parameters (infer_state.sampling) the token comes from the
 sampling kernel instead of argmax.  With a sharded lm_head, batches without top-k / top-p sample each shard and exchange
 (best score, global index) pairs through the same all-gather - the noise is keyed by the global index, so the merged token is
-the unsharded one; otherwise the logits are all-gathered and every rank samples the full rows."""
+the unsharded one; otherwise the logits are all-gathered and every rank samples the full rows.
+
+Addition (log-probabilities, csrc/logprobs.cu): when the step asks for them (infer_state.logprobs = N), the log-probability of
+the chosen token and the top-N entries are computed from the same logits the token was chosen from, and the layer returns
+(tokens, token logprobs, top ids, top logprobs).  With a sharded lm_head the full rows are gathered first, so every rank
+chooses the token and computes identical log-probabilities from whole rows."""
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.linear import linear
+from swiftllm_b200.worker.kernels.logprobs import token_logprobs
 from swiftllm_b200.worker.kernels.rmsnorm import rmsnorm_inplace
 from swiftllm_b200.worker.kernels.sampling import sample_tokens
 
@@ -50,20 +56,27 @@ class LlamaPostLayer:
         if not already_normed:
             rmsnorm_inplace(last_input, self.weights.final_norm, self.model_config.rms_norm_eps)
         logits = linear(last_input, self.weights.lm_head)      # [batch_size, vocab_size] (or this rank's V / tp_size columns)
-        sp = infer_state.sampling
+        sp, n = infer_state.sampling, infer_state.logprobs
         if not self.sharded:
             if self.keep_logits:
                 self.last_logits = logits
             if sp is not None:
-                return sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
-            return torch.argmax(logits, dim=1)
+                tokens = sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+            else:
+                tokens = torch.argmax(logits, dim=1)
+            return tokens if n is None else (tokens,) + token_logprobs(logits, tokens, n)
 
         B, Vs = logits.shape
-        if sp is not None and sp.filtered:                     # top-k / top-p need whole rows: gather them, sample on every rank
+        if (sp is not None and sp.filtered) or n is not None:
+            # top-k / top-p and log-probabilities need whole rows: gather them, choose the token on every rank
             full = self._gather_logits(logits)
             if self.keep_logits:
                 self.last_logits = full
-            return sample_tokens(full, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+            if sp is not None:
+                tokens = sample_tokens(full, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+            else:
+                tokens = torch.argmax(full, dim=1)
+            return tokens if n is None else (tokens,) + token_logprobs(full, tokens, n)
         if sp is not None:
             mine = torch.empty((B, 2), dtype=torch.float32, device=logits.device)
             sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos, vocab_offset=self.tp_rank * Vs,

@@ -3,6 +3,7 @@
 
     LlamaModel(engine_config) -> load_weights() -> profile_num_blocks() -> init_kvcache_and_swap(num_blocks)
     forward(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False) -> list[int]
+    forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities)
     swap_in_seqs / swap_out_seqs / free_seqs_resources
 
 and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).
@@ -25,7 +26,7 @@ import torch.distributed as dist
 from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
-from swiftllm_b200.sampling_params import sampling_words
+from swiftllm_b200.sampling_params import TokenLogprobs, logprobs_top_n, sampling_words
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.weight import load_weights
@@ -317,9 +318,41 @@ class LlamaModel:
     def forward_async(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False,
                       prefill_prefix_lens_list=None, sampling_params_list=None) -> torch.Tensor:
         """Same as forward() but returns the token tensor on the device (no sync)."""
+        return self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
+                          sampling_params_list, with_logprobs=False)
+
+    @torch.inference_mode()
+    def forward_with_logprobs(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
+                              ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
+                              sampling_params_list: Optional[list] = None) -> list:
+        """forward() that also returns log-probabilities: one swiftllm_b200.TokenLogprobs(token, logprob, top) per batch entry.
+        Entry i gets them when sampling_params_list[i].logprobs is not None: the log-probability of its token and, for
+        logprobs = N > 0, the N most likely tokens as (id, logprob), most likely first, ties broken by the smaller id.  They are
+        log_softmax of the raw logits the token was chosen from (csrc/logprobs.cu), not of the temperature-scaled or filtered
+        distribution.  The tokens are the ones forward() returns for the same arguments."""
+        out = self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
+                         sampling_params_list, with_logprobs=True)
+        if isinstance(out, torch.Tensor):                   # no entry asked: forward()'s step
+            return [TokenLogprobs(t) for t in out.tolist()]
+        tokens, token_lp, top_ids, top_lp = (t.tolist() for t in out)
+        res = []
+        for i, t in enumerate(tokens):
+            n = sampling_params_list[i].logprobs
+            if n is None:
+                res.append(TokenLogprobs(t))
+            else:
+                n = min(int(n), self.model_config.vocab_size)
+                res.append(TokenLogprobs(t, token_lp[i], list(zip(top_ids[i][:n], top_lp[i][:n]))))
+        return res
+
+    def _step(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
+              sampling_params_list, with_logprobs: bool):
+        """One step: the token tensor, or with log-probabilities asked for by some entry (with_logprobs and a
+        SamplingParams.logprobs set) the tuple (tokens, token logprobs, top ids, top logprobs) on the device."""
         mc = self.model_config
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
+        top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
         num_prefill_seqs = len(input_ids_list) - len(decoding_seq_lens_list)
         flat_ids = list(itertools.chain(*input_ids_list))
         prefill_lens = [len(s) for s in input_ids_list[:num_prefill_seqs]]
@@ -346,7 +379,8 @@ class LlamaModel:
 
         if (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
                 and batch_size > 0):
-            return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp)
+            return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
+                                              top_n)
 
         # the sampling words go first: the int64 seeds need an 8-byte aligned offset
         views = self._stage_metadata(
@@ -378,16 +412,17 @@ class LlamaModel:
             paged_attn_seq_block_size=0, last_token_indices=last,
             prefill_prefix_lens=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0,
-            sampling=sampling,
+            sampling=sampling, logprobs=top_n,
         )
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
-    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None):
+    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None):
         """Pure-decode step replayed from a CUDA graph.  Static device buffers hold the step's metadata; the graph
         (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
         allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
-        filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy."""
+        filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy.  A step
+        with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel."""
         from swiftllm_b200 import _lib
         B = len(flat_ids)
         mc = self.model_config
@@ -400,6 +435,8 @@ class LlamaModel:
         if samp:
             # sharded lm_head: filtered rows sample the gathered full rows, the others exchange per-shard pairs
             key += (True, samp[1] and self.post_layer.sharded)
+        if top_n is not None:
+            key += ("logprobs", top_n)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -407,7 +444,7 @@ class LlamaModel:
             cap = max(1, int(getattr(self.engine_config, "max_cuda_graphs", 16)))
             while len(self._graphs) >= cap:
                 self._graphs.pop(next(iter(self._graphs)))
-            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1])
+            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n)
         self._graphs[key] = g                    # (re)insert as most recently used
         # host-side bookkeeping of the allocator (exhaustion check + mirror), no device work here
         bm = self.gpu_block_manager
@@ -435,11 +472,14 @@ class LlamaModel:
         ev.record()
         self._wait_for_swaps()
         g["graph"].replay()
-        # the graph's static output is overwritten by the next replay: hand out a copy (stream-ordered, no sync)
+        # the graph's static outputs are overwritten by the next replay: hand out copies (stream-ordered, no sync)
+        if g["logprobs"] is not None:
+            return (g["tokens"].clone(),) + tuple(t.clone() for t in g["logprobs"])
         return g["tokens"].clone()
 
-    def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None):
-        """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words."""
+    def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None):
+        """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
+        also computes log-probabilities with this top-N."""
         from swiftllm_b200.worker.kernels.block_mgmt import allocate_blocks_for_seqs as alloc_kernel
         mc, ec = self.model_config, self.engine_config
         dev = self.device
@@ -462,7 +502,7 @@ class LlamaModel:
                 num_decoding_seqs=B, decoding_seq_lens=lens, max_decoding_len=bucket_len,
                 seq_block_size=2048, num_seq_blocks=(bucket_len + 2047) // 2048,
                 position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=sampling)
+                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=sampling, logprobs=top_n)
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
@@ -486,10 +526,11 @@ class LlamaModel:
         if getattr(self, "_graph_pool", None) is None:
             self._graph_pool = torch.cuda.graph_pool_handle()
         with torch.cuda.graph(graph, pool=self._graph_pool):
-            tokens = step(self.gpu_block_manager, self.k_cache, self.v_cache)
+            out = step(self.gpu_block_manager, self.k_cache, self.v_cache)
         torch.cuda.synchronize()
+        tokens, logprobs = (out, None) if top_n is None else (out[0], out[1:])
         # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph
-        return dict(graph=graph, meta=meta, host=host, next=0, tokens=tokens, keep=(last, empty))
+        return dict(graph=graph, meta=meta, host=host, next=0, tokens=tokens, logprobs=logprobs, keep=(last, empty))
 
     # ------------------------------------------------------------------ swap / free
     def _swap(self, seq_ids_list: list, is_swap_in: bool):
