@@ -9,6 +9,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --cuda-graph       replay decode steps from CUDA graphs
     ... --temperature 0.8 --top-p 0.95 [--top-k 50] [--seed 1]    sample instead of greedy decoding
     ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
+    ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
 """
 import argparse
 import os
@@ -84,6 +85,9 @@ def main():
     ap.add_argument("--top-p", type=float, default=1.0, help="keep the smallest set of tokens with this much mass (1 = off)")
     ap.add_argument("--seed", type=int, default=None, help="sampling seed (default: a fresh one per step from the engine's generator)")
     ap.add_argument("--logprobs", type=int, default=None, help="print each token's log-probability and the N most likely tokens (0..20)")
+    ap.add_argument("--repetition-penalty", type=float, default=1.0, help="divide / multiply the logits of seen tokens (1 = off)")
+    ap.add_argument("--frequency-penalty", type=float, default=0.0, help="subtract this times each token's output count (0 = off)")
+    ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
     args = ap.parse_args()
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
@@ -112,14 +116,17 @@ def main():
     model.init_kvcache_and_swap(num_blocks)
     print(f"{num_blocks} KV blocks; model ready in {time.perf_counter() - t0:.1f} s")
 
-    params = None if args.temperature == 0 and args.logprobs is None else \
-        swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs)
+    params = swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs,
+                                          repetition_penalty=args.repetition_penalty, frequency_penalty=args.frequency_penalty,
+                                          presence_penalty=args.presence_penalty)
+    if args.temperature == 0 and args.logprobs is None and not params.has_penalties():
+        params = None
     logs = [[] for _ in input_ids]
     outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs)
     seq_ids = list(range(len(input_ids)))
     for p, o, lg in zip(input_ids, outputs, logs):
         print(f"[{len(p)} prompt tokens] -> {show(o)}")
-        for r in lg:      # log-probabilities of the raw model distribution (before temperature / top-k / top-p)
+        for r in lg:      # log-probabilities of the raw model distribution (before penalties, temperature / top-k / top-p)
             top = ", ".join(f"{show([t])!r}:{lp:.3f}" for t, lp in r.top)
             print(f"    {show([r.token])!r} {r.logprob:.4f}   top [{top}]")
     print(f"prefill {t_prefill * 1e3:.1f} ms ({sum(map(len, input_ids)) / t_prefill:.0f} tok/s), "

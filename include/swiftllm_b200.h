@@ -244,6 +244,28 @@ int sllm_token_logprobs(const void* logits, int64_t num_rows, int vocab_size, in
                         const int64_t* token_ids, int top_n, float* out_token_logprob, int32_t* out_top_ids,
                         float* out_top_logprobs, sllm_dtype_t dtype, sllm_stream_t stream);
 
+/* ---- Repetition / frequency / presence penalties (new; the reference has no sampling controls), IN PLACE on logits laid out
+ * as in sllm_sample_tokens (a vocabulary shard with vocab_offset works).  Per-row DEVICE arrays [num_rows]:
+ * repetition_penalty, frequency_penalty, presence_penalty (a row with 1, 0, 0 is skipped: nothing read, recorded or modified),
+ * seq_ids (block-table rows), pos (the sequence length after this step's input).  The row's history is positions [0, pos) of its
+ * sequence: [0, pos - n_new) read from token_cache int32 [num_blocks, block_size] through block_table int32
+ * [*, block_table_stride] (entries id | is_output << 31), the rest its n_new new tokens in input_ids: rows below
+ * num_prefill_rows are prefill entries (n_new = prefill_seq_lens[i] prompt tokens ending at input_ids[last_token_indices[i]]),
+ * the others decode rows (one output token, input_ids[last_token_indices[i]]).  For every id v of the shard seen in the history:
+ * l = l > 0 ? l / r : l * r, then l -= f * c_out(v) + (c_out(v) > 0 ? p : 0), c_out counting output tokens, fp32 without
+ * contraction and one rounding to the storage dtype; other entries keep their bits.  The new tokens are then written to
+ * positions [pos - n_new, pos) of the pages.  Ids outside the shard, unmapped positions and block ids outside [0, num_blocks)
+ * are skipped.  Deterministic (exact integer counts).  Rejected before launch: unknown dtype, vocab_size <= 0 or larger than 8
+ * shared-memory slices of 4-byte slots (about 409k entries), global indices >= 2^31, a row stride below vocab_size, block_size
+ * outside [1, 65536], a bad block_table_stride, num_blocks < 0, num_prefill_rows outside [0, num_rows], num_rows outside
+ * [0, 2^20], null pointers (prefill_seq_lens may be NULL when num_prefill_rows is 0). */
+int sllm_apply_penalties(void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride, int64_t vocab_offset,
+                         const float* repetition_penalty, const float* frequency_penalty, const float* presence_penalty,
+                         const int32_t* seq_ids, const int32_t* pos, const int32_t* input_ids,
+                         const int32_t* last_token_indices, const int32_t* prefill_seq_lens, int num_prefill_rows,
+                         const int32_t* block_table, int block_table_stride, int block_size, int32_t* token_cache,
+                         int64_t num_blocks, sllm_dtype_t dtype, sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,13 +16,22 @@ class SamplingParams:
     function of the logits, the parameters and the sequence length only.
 
     logprobs (LlamaModel.forward_with_logprobs): None returns none, 0 the returned token's log-probability, 1..20 also the
-    top-N alternatives.  They are log_softmax of the raw logits - the model's distribution before temperature, top-k and top-p.
-    forward / forward_async ignore the field."""
+    top-N alternatives.  They are log_softmax of the raw logits - the model's distribution before penalties, temperature, top-k and
+    top-p; a penalised greedy token therefore need not be top[0].  forward / forward_async ignore the field.
+
+    Penalties (csrc/penalties.cu; the order and formulas of vLLM), applied to the logits before greedy argmax or sampling, in fp32:
+    repetition_penalty r (1: off) divides a positive logit / multiplies a non-positive one of every token seen in the prompt or
+    the output; then frequency_penalty f and presence_penalty p (0: off) subtract f * count + p from every token that occurs
+    count > 0 times in the output.  The history is read from the token pages the model records in steps where a row carries
+    penalties, so a request that uses them must pass the same SamplingParams from its first prefill chunk on."""
     temperature: float = 0.0
     top_k: int = 0
     top_p: float = 1.0
     seed: Optional[int] = None
     logprobs: Optional[int] = None
+    repetition_penalty: float = 1.0
+    frequency_penalty: float = 0.0
+    presence_penalty: float = 0.0
 
     def validate(self):
         if not (isinstance(self.temperature, (int, float)) and math.isfinite(self.temperature) and self.temperature >= 0):
@@ -37,6 +46,19 @@ class SamplingParams:
         if self.logprobs is not None and (isinstance(self.logprobs, bool) or not isinstance(self.logprobs, (int, np.integer))
                                           or not 0 <= self.logprobs <= MAX_LOGPROBS):
             raise ValueError(f"logprobs must be None or an integer in [0, {MAX_LOGPROBS}], got {self.logprobs!r}")
+        if not (_is_real(self.repetition_penalty) and math.isfinite(self.repetition_penalty) and self.repetition_penalty > 0):
+            raise ValueError(f"repetition_penalty must be a finite number > 0, got {self.repetition_penalty!r}")
+        for name in ("frequency_penalty", "presence_penalty"):
+            v = getattr(self, name)
+            if not (_is_real(v) and math.isfinite(v) and -2 <= v <= 2):
+                raise ValueError(f"{name} must be a finite number in [-2, 2], got {v!r}")
+
+    def has_penalties(self) -> bool:
+        return self.repetition_penalty != 1.0 or self.frequency_penalty != 0.0 or self.presence_penalty != 0.0
+
+
+def _is_real(v) -> bool:
+    return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool)
 
 
 class TokenLogprobs(NamedTuple):
@@ -60,7 +82,8 @@ def _i32(words: np.ndarray) -> list:
 
 def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator):
     """Validates the list and returns the staged int32 words (seed lo/hi interleaved [2B], temperature bits [B], top_k [B],
-    top_p bits [B]) and whether any row filters (top-k / top-p); None when every row is greedy.  Raises ValueError."""
+    top_p bits [B], and when some row has penalties the fp32 bits of repetition, frequency and presence penalty [3B]) and whether
+    any row filters (top-k / top-p); None when every row is greedy and none has penalties.  Raises ValueError."""
     if len(params_list) != batch_size:
         raise ValueError(f"sampling_params_list has {len(params_list)} entries for a batch of {batch_size}")
     for sp in params_list:
@@ -69,11 +92,20 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
         sp.validate()
     # a fresh seed for every unseeded row, drawn even for greedy rows so the stream does not depend on the batch's mix
     seeds = np.array([int(rng.integers(0, 2 ** 63)) if sp.seed is None else int(sp.seed) for sp in params_list], dtype=np.uint64)
-    if all(sp.temperature == 0 for sp in params_list):
+    penalized = any(sp.has_penalties() for sp in params_list)
+    if not penalized and all(sp.temperature == 0 for sp in params_list):
         return None
     temp = np.array([sp.temperature for sp in params_list], dtype=np.float32)
     top_p = np.array([sp.top_p for sp in params_list], dtype=np.float32)
     top_k = [int(sp.top_k) for sp in params_list]
     filtered = any(sp.temperature > 0 and (sp.top_k > 0 or sp.top_p < 1) for sp in params_list)
     words = _i32(seeds.view(np.uint32)) + _i32(temp.view(np.uint32)) + top_k + _i32(top_p.view(np.uint32))
+    if penalized:
+        for name in ("repetition_penalty", "frequency_penalty", "presence_penalty"):
+            words += _i32(np.array([getattr(sp, name) for sp in params_list], dtype=np.float32).view(np.uint32))
     return words, filtered
+
+
+def has_penalties(params_list: Optional[list]) -> bool:
+    """Some entry of the (validated) list has a penalty: the step applies them and records its tokens in the token pages."""
+    return any(sp.has_penalties() for sp in params_list or [])

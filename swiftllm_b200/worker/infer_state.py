@@ -64,11 +64,31 @@ class SamplingState:
     seed: torch.Tensor              # [batch_size] int64
     pos: torch.Tensor               # [batch_size] int32: sequence length after this step's input (noise counter)
     filtered: bool                  # some row uses top-k or top-p (needs the whole vocabulary row on one rank)
+    # ---- penalties (csrc/penalties.cu); None when no row of the step has any
+    repetition_penalty: Optional[torch.Tensor] = None   # [batch_size] float32, 1 = off
+    frequency_penalty: Optional[torch.Tensor] = None    # [batch_size] float32, 0 = off
+    presence_penalty: Optional[torch.Tensor] = None     # [batch_size] float32, 0 = off
+    sampled: bool = True            # some row has temperature > 0; False: every row takes the argmax of its penalised logits
+    # the token history the penalty kernel reads and extends, set by the model: the step's input ids (int32 [num_tokens]), the
+    # block table and the token pages (int32 [num_blocks, block_size])
+    input_ids: Optional[torch.Tensor] = None
+    block_table: Optional[torch.Tensor] = None
+    token_cache: Optional[torch.Tensor] = None
+
+    @property
+    def penalized(self) -> bool:
+        return self.repetition_penalty is not None
 
     @staticmethod
-    def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool) -> "SamplingState":
-        """`words`: the int32 device view staged from swiftllm_b200.sampling_params.sampling_words (8-byte aligned)."""
+    def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool, sampled: bool = True) -> "SamplingState":
+        """`words`: the int32 device view staged from swiftllm_b200.sampling_params.sampling_words (8-byte aligned); 8 * B
+        words carry the penalties after the 5 * B sampling words."""
         B = pos.shape[0]
+        pen = {}
+        if words.shape[0] == 8 * B:
+            pen = dict(repetition_penalty=words[5 * B:6 * B].view(torch.float32),
+                       frequency_penalty=words[6 * B:7 * B].view(torch.float32),
+                       presence_penalty=words[7 * B:8 * B].view(torch.float32))
         return SamplingState(temperature=words[2 * B:3 * B].view(torch.float32), top_k=words[3 * B:4 * B],
                              top_p=words[4 * B:5 * B].view(torch.float32), seed=words[:2 * B].view(torch.int64), pos=pos,
-                             filtered=filtered)
+                             filtered=filtered, sampled=sampled, **pen)

@@ -12,13 +12,20 @@ the unsharded one; otherwise the logits are all-gathered and every rank samples 
 Addition (log-probabilities, csrc/logprobs.cu): when the step asks for them (infer_state.logprobs = N), the log-probability of
 the chosen token and the top-N entries are computed from the same logits the token was chosen from, and the layer returns
 (tokens, token logprobs, top ids, top logprobs).  With a sharded lm_head the full rows are gathered first, so every rank
-chooses the token and computes identical log-probabilities from whole rows."""
+chooses the token and computes identical log-probabilities from whole rows.
+
+Addition (penalties, csrc/penalties.cu): when some row carries repetition / frequency / presence penalties (sampling.penalized),
+the logits the token is chosen from are penalised first (a copy when log-probabilities are asked for: they stay those of the raw
+logits) and the step's tokens are recorded in the token pages.  With a sharded lm_head the pair-merge path penalises each rank's
+shard (vocab_offset) before its local choice; the gather path penalises the gathered full rows on every rank.  Every rank records
+the same tokens in its own pages."""
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.linear import linear
 from swiftllm_b200.worker.kernels.logprobs import token_logprobs
+from swiftllm_b200.worker.kernels.penalties import apply_penalties
 from swiftllm_b200.worker.kernels.rmsnorm import rmsnorm_inplace
 from swiftllm_b200.worker.kernels.sampling import sample_tokens
 
@@ -57,13 +64,16 @@ class LlamaPostLayer:
             rmsnorm_inplace(last_input, self.weights.final_norm, self.model_config.rms_norm_eps)
         logits = linear(last_input, self.weights.lm_head)      # [batch_size, vocab_size] (or this rank's V / tp_size columns)
         sp, n = infer_state.sampling, infer_state.logprobs
+        pen = sp is not None and sp.penalized
+        sampled = sp is not None and sp.sampled
         if not self.sharded:
             if self.keep_logits:
-                self.last_logits = logits
-            if sp is not None:
-                tokens = sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+                self.last_logits = logits.clone() if pen else logits
+            chosen = self._penalised(logits, infer_state, idx, copy=n is not None) if pen else logits
+            if sampled:
+                tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
             else:
-                tokens = torch.argmax(logits, dim=1)
+                tokens = torch.argmax(chosen, dim=1)
             return tokens if n is None else (tokens,) + token_logprobs(logits, tokens, n)
 
         B, Vs = logits.shape
@@ -71,13 +81,17 @@ class LlamaPostLayer:
             # top-k / top-p and log-probabilities need whole rows: gather them, choose the token on every rank
             full = self._gather_logits(logits)
             if self.keep_logits:
-                self.last_logits = full
-            if sp is not None:
-                tokens = sample_tokens(full, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+                self.last_logits = full.clone() if pen else full
+            chosen = self._penalised(full, infer_state, idx, copy=n is not None) if pen else full
+            if sampled:
+                tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
             else:
-                tokens = torch.argmax(full, dim=1)
+                tokens = torch.argmax(chosen, dim=1)
             return tokens if n is None else (tokens,) + token_logprobs(full, tokens, n)
-        if sp is not None:
+        raw_full = self._gather_logits(logits) if self.keep_logits and pen else None
+        if pen:
+            self._penalised(logits, infer_state, idx, copy=False, vocab_offset=self.tp_rank * Vs)
+        if sampled:
             mine = torch.empty((B, 2), dtype=torch.float32, device=logits.device)
             sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos, vocab_offset=self.tp_rank * Vs,
                           out_pairs=mine)
@@ -89,8 +103,19 @@ class LlamaPostLayer:
         pairs = torch.empty((self.tp_size * B, 2), dtype=torch.float32, device=logits.device)
         dist.all_gather_into_tensor(pairs, mine.contiguous(), group=self.tp_group)
         if self.keep_logits:                                   # parity tests only: reassemble the full logits
-            self.last_logits = self._gather_logits(logits)
+            self.last_logits = raw_full if raw_full is not None else self._gather_logits(logits)
         return merge_sharded_argmax(pairs.view(self.tp_size, B, 2))
+
+    @staticmethod
+    def _penalised(logits: torch.Tensor, infer_state: LlamaInferState, last_idx: torch.Tensor, copy: bool,
+                   vocab_offset: int = 0) -> torch.Tensor:
+        """The penalised logits (in place, or a copy), the step's tokens recorded in the token pages."""
+        sp = infer_state.sampling
+        out = logits.clone() if copy else logits
+        apply_penalties(out, sp.repetition_penalty, sp.frequency_penalty, sp.presence_penalty, sp.pos, infer_state.seq_ids,
+                        sp.input_ids, last_idx, infer_state.prefill_seq_lens, infer_state.num_prefill_seqs, sp.block_table,
+                        sp.token_cache, vocab_offset=vocab_offset)
+        return out
 
     def _gather_logits(self, logits: torch.Tensor) -> torch.Tensor:
         """[B, V / tp_size] shards of every rank -> [B, V] (vocabulary order)."""

@@ -6,7 +6,8 @@
     forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities)
     swap_in_seqs / swap_out_seqs / free_seqs_resources
 
-and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).
+and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).  Addition: the token
+pages token_cache / token_swap (int32 [blocks, block_size], id | is_output << 31), the history the penalty kernel reads.
 
 Host path (SURVEY.md §8 f-2): all per-step metadata travels in ONE pinned staging buffer and one
 H2D copy (the reference issues ~6 small copies, model.py:272-297); block allocation is one sync-free kernel
@@ -15,6 +16,7 @@ from a CUDA graph; the only sync of a step is the final `.tolist()` of the sampl
 """
 from __future__ import annotations
 
+import dataclasses
 import itertools
 import math
 from typing import Callable, Optional
@@ -26,7 +28,7 @@ import torch.distributed as dist
 from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
-from swiftllm_b200.sampling_params import TokenLogprobs, logprobs_top_n, sampling_words
+from swiftllm_b200.sampling_params import TokenLogprobs, has_penalties, logprobs_top_n, sampling_words
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.weight import load_weights
@@ -99,6 +101,9 @@ class LlamaModel:
         self.num_blocks = None
         self.k_cache = self.v_cache = None
         self.k_swap = self.v_swap = None
+        # token pages (SamplingParams penalties): written in steps with a penalised row, carried in swaps once one has run
+        self.token_cache = self.token_swap = None
+        self._penalties_used = False
         self.cpu_block_manager = self.gpu_block_manager = None
         self.tp_group = None
         self._graphs = {}
@@ -227,6 +232,10 @@ class LlamaModel:
         pin = bool(getattr(ec, "pin_swap_space", True)) and ec.num_cpu_blocks > 0
         self.k_swap = torch.zeros(sshape, dtype=self.dtype, device="cpu", pin_memory=pin)
         self.v_swap = torch.zeros(sshape, dtype=self.dtype, device="cpu", pin_memory=pin)
+        # 4 B per token; left uninitialised (no device work): a position is always written before a penalised step reads it
+        self.token_cache = torch.empty((num_blocks, ec.block_size), dtype=torch.int32, device=self.device)
+        self.token_swap = torch.empty((ec.num_cpu_blocks, ec.block_size), dtype=torch.int32, device="cpu", pin_memory=pin)
+        self._penalties_used = False
         self.gpu_block_manager = BlockManager("GPU", num_blocks, ec.max_seqs_in_block_table, ec.max_blocks_per_seq,
                                               ec.block_size, device=self.device)
         self.cpu_block_manager = BlockManager("CPU", ec.num_cpu_blocks, ec.max_seqs_in_block_table,
@@ -309,8 +318,10 @@ class LlamaModel:
 
         `sampling_params_list` (addition): one swiftllm_b200.SamplingParams per batch entry; the token of entry i is drawn with
         its temperature / top-k / top-p and seed (csrc/sampling.cu), the noise keyed by the sequence length after this step.
-        None (or every temperature 0) is greedy decoding, the reference's behaviour.  Invalid parameters raise ValueError
-        before anything is enqueued."""
+        None (or every temperature 0) is greedy decoding, the reference's behaviour.  Entries with repetition / frequency /
+        presence penalties have their logits penalised first (csrc/penalties.cu), over the history recorded in the token pages:
+        such a request must carry the same parameters from its first prefill chunk on.  Invalid parameters (and penalties with
+        ignore_kvcache, which has no block table to record into) raise ValueError before anything is enqueued."""
         return self.forward_async(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache,
                                   prefill_prefix_lens_list, sampling_params_list).tolist()
 
@@ -353,6 +364,10 @@ class LlamaModel:
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
+        penalized = has_penalties(sampling_params_list)
+        if penalized and ignore_kvcache:
+            raise ValueError("penalties need the token history of the block table: not available with ignore_kvcache")
+        sampled = samp is not None and any(sp.temperature > 0 for sp in sampling_params_list)
         num_prefill_seqs = len(input_ids_list) - len(decoding_seq_lens_list)
         flat_ids = list(itertools.chain(*input_ids_list))
         prefill_lens = [len(s) for s in input_ids_list[:num_prefill_seqs]]
@@ -380,7 +395,7 @@ class LlamaModel:
         if (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
                 and batch_size > 0):
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
-                                              top_n)
+                                              top_n, penalized, sampled)
 
         # the sampling words go first: the int64 seeds need an 8-byte aligned offset
         views = self._stage_metadata(
@@ -388,6 +403,10 @@ class LlamaModel:
             last_idx, prefix_lens if chunked else [])
         ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = views[-8:]
         sampling = SamplingState.from_staged(views[0], seq_lengths, samp[1]) if samp else None
+        if penalized:
+            sampling = dataclasses.replace(sampling, sampled=sampled, input_ids=ids,
+                                           block_table=self.gpu_block_manager.block_table, token_cache=self.token_cache)
+            self._penalties_used = True
 
         if not ignore_kvcache:
             self.gpu_block_manager.allocate_blocks_for_seqs(seq_ids, seq_lengths, seq_ids_list=seq_ids_list,
@@ -417,12 +436,14 @@ class LlamaModel:
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
-    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None):
+    def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
+                              sampled=True):
         """Pure-decode step replayed from a CUDA graph.  Static device buffers hold the step's metadata; the graph
         (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
         allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
         filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy.  A step
-        with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel."""
+        with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
+        penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples)."""
         from swiftllm_b200 import _lib
         B = len(flat_ids)
         mc = self.model_config
@@ -437,6 +458,8 @@ class LlamaModel:
             key += (True, samp[1] and self.post_layer.sharded)
         if top_n is not None:
             key += ("logprobs", top_n)
+        if penalized:
+            key += ("penalties", sampled)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -444,7 +467,7 @@ class LlamaModel:
             cap = max(1, int(getattr(self.engine_config, "max_cuda_graphs", 16)))
             while len(self._graphs) >= cap:
                 self._graphs.pop(next(iter(self._graphs)))
-            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n)
+            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled)
         self._graphs[key] = g                    # (re)insert as most recently used
         # host-side bookkeeping of the allocator (exhaustion check + mirror), no device work here
         bm = self.gpu_block_manager
@@ -465,33 +488,39 @@ class LlamaModel:
         ev.synchronize()
         hv = host.numpy()
         if samp:
-            hv[:5 * B] = samp[0]
-            hv = hv[5 * B:]
+            nw = len(samp[0])                   # 5 * B sampling words, 8 * B with penalties
+            hv[:nw] = samp[0]
+            hv = hv[nw:]
         hv[:B] = flat_ids; hv[B:2 * B] = seq_ids_list; hv[2 * B:3 * B] = lens_list
         g["meta"].copy_(host, non_blocking=True)
         ev.record()
         self._wait_for_swaps()
+        self._penalties_used |= penalized
         g["graph"].replay()
         # the graph's static outputs are overwritten by the next replay: hand out copies (stream-ordered, no sync)
         if g["logprobs"] is not None:
             return (g["tokens"].clone(),) + tuple(t.clone() for t in g["logprobs"])
         return g["tokens"].clone()
 
-    def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None):
+    def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None,
+                              penalized: bool = False, sampled: bool = True):
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
-        also computes log-probabilities with this top-N."""
+        also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
+        the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax."""
         from swiftllm_b200.worker.kernels.block_mgmt import allocate_blocks_for_seqs as alloc_kernel
         mc, ec = self.model_config, self.engine_config
         dev = self.device
-        nw = 0 if filtered is None else 5 * B
+        nw = 0 if filtered is None else (8 if penalized else 5) * B
         meta = torch.zeros((nw + 3 * B,), dtype=torch.int32, device=dev)
         host = [(torch.zeros((nw + 3 * B,), dtype=torch.int32).pin_memory(), torch.cuda.Event()) for _ in range(self._STAGE_SLOTS)]
         ids, seq_ids, lens = meta[nw:nw + B], meta[nw + B:nw + 2 * B], meta[nw + 2 * B:]
-        sampling = None if filtered is None else SamplingState.from_staged(meta[:nw], lens, filtered)
+        sampling = None if filtered is None else SamplingState.from_staged(meta[:nw], lens, filtered, sampled)
         last = torch.arange(B, dtype=torch.int32, device=dev)
         empty = torch.empty((0,), dtype=torch.int32, device=dev)
 
-        def step(bm, k_cache, v_cache):
+        def step(bm, k_cache, v_cache, token_cache):
+            samp_state = sampling if not penalized else \
+                dataclasses.replace(sampling, input_ids=ids, block_table=bm.block_table, token_cache=token_cache)
             alloc_kernel(bm.num_seq_allocated_blocks, bm.block_table, bm.is_block_free, seq_ids, lens, bm.block_size,
                          None, bm._status)
             pos = (lens - 1).long()
@@ -502,7 +531,8 @@ class LlamaModel:
                 num_decoding_seqs=B, decoding_seq_lens=lens, max_decoding_len=bucket_len,
                 seq_block_size=2048, num_seq_blocks=(bucket_len + 2047) // 2048,
                 position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=sampling, logprobs=top_n)
+                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=samp_state,
+                logprobs=top_n)
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
@@ -511,6 +541,7 @@ class LlamaModel:
         sshape = (B,) + tuple(self.k_cache.shape[1:])
         k_s = torch.zeros(sshape, dtype=self.dtype, device=dev)
         v_s = torch.zeros(sshape, dtype=self.dtype, device=dev)
+        t_s = torch.zeros((B, ec.block_size), dtype=torch.int32, device=dev) if penalized else None
         meta.zero_()
         seq_ids.copy_(torch.arange(B, dtype=torch.int32, device=dev))
         lens.fill_(1)
@@ -518,15 +549,15 @@ class LlamaModel:
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
             for _ in range(2):
-                step(scratch_bm, k_s, v_s)
+                step(scratch_bm, k_s, v_s, t_s)
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
-        del k_s, v_s, scratch_bm
+        del k_s, v_s, t_s, scratch_bm
         graph = torch.cuda.CUDAGraph()
         if getattr(self, "_graph_pool", None) is None:
             self._graph_pool = torch.cuda.graph_pool_handle()
         with torch.cuda.graph(graph, pool=self._graph_pool):
-            out = step(self.gpu_block_manager, self.k_cache, self.v_cache)
+            out = step(self.gpu_block_manager, self.k_cache, self.v_cache, self.token_cache)
         torch.cuda.synchronize()
         tokens, logprobs = (out, None) if top_n is None else (out[0], out[1:])
         # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph
@@ -554,6 +585,7 @@ class LlamaModel:
         if not getattr(self.engine_config, "swap_on_copy_stream", False):
             # ids stay on the device (device_swap): one gather/scatter kernel over the mapped swap space, sync-free
             copy(src_ids, dst_ids, is_swap_in, self.k_cache, self.v_cache, self.k_swap, self.v_swap)
+            self._swap_token_pages(copy, src_ids, dst_ids, is_swap_in)
             return
         # copy stream: the copy starts once everything enqueued so far on this stream (the block-table kernels above, the KV
         # stores of earlier steps) has finished; the next forward waits for `_swap_done` before it touches the cache
@@ -564,10 +596,18 @@ class LlamaModel:
         with torch.cuda.stream(self._swap_stream):
             self._swap_stream.wait_event(ready)
             copy(src_ids, dst_ids, is_swap_in, self.k_cache, self.v_cache, self.k_swap, self.v_swap)
+            self._swap_token_pages(copy, src_ids, dst_ids, is_swap_in)
             if device_ids and src_ids.is_cuda:       # the id tensors were allocated on the main stream
                 src_ids.record_stream(self._swap_stream); dst_ids.record_stream(self._swap_stream)
             self._swap_done = torch.cuda.Event()
             self._swap_done.record()
+
+    def _swap_token_pages(self, copy, src_ids, dst_ids, is_swap_in: bool):
+        """The token pages follow their KV blocks through the same id lists, once a penalised step has run (a run without
+        penalties swaps exactly what it did before).  The swap entry points move a (k, v) pair: the one table goes in as both,
+        so its 4 B per token are copied twice."""
+        if self._penalties_used:
+            copy(src_ids, dst_ids, is_swap_in, self.token_cache, self.token_cache, self.token_swap, self.token_swap)
 
     @torch.inference_mode()
     def swap_in_seqs(self, seq_ids_list: list):
