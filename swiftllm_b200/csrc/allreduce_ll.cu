@@ -18,7 +18,11 @@
 // rank pushes into a peer's line only after it finished the previous exchange that used the line, which needed every row that
 // peer owns - rows the peer produced AFTER consuming the line; an owner's broadcast needs this exchange's pushes of every rank,
 // i.e. everybody has finished the previous one (tests/test_ll_exchange_protocol_sim.py checks every interleaving it can find).
-// Every CTA of the grid must be co-resident (they wait for peers): grid <= 2 CTAs per SM, rows are looped.
+// Residency: the grid is min(T, 2 x SMs) CTAs, rows are looped.  That is NOT always one wave: the kernel needs 126 (fp16) / 128
+// (bf16) registers per thread, so at 512 threads (H >= 4096) only one CTA fits per SM and T > SMs runs in two waves.  It cannot
+// deadlock as long as each GPU dispatches CTAs in increasing blockIdx order: grid and row-to-CTA map are the same on every rank,
+// so in all three phases CTA c waits only for CTA c of each peer, and the lowest CTA index still unfinished anywhere is then
+// resident on every rank where it has not finished.
 #include <type_traits>
 
 #include "common.cuh"
@@ -227,7 +231,7 @@ extern "C" int sllm_allreduce_add_rmsnorm_ll(const void* partial, void* const* h
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         sm_count[dev] = n > 0 ? n : 132;
     }
-    const int64_t cap = 2LL * sm_count[dev];                         // every CTA must be resident: 2 x 512 threads per SM always fit
+    const int64_t cap = 2LL * sm_count[dev];                         // one wave below 512 threads, two at 512: see the kernel comment
     const unsigned grid = (unsigned)(num_tokens < cap ? num_tokens : cap);
     cudaStream_t st = (cudaStream_t)stream;
     const bool nvls = mc_ag_recv != nullptr;

@@ -9,7 +9,8 @@ exchange kernel -> consumer, alternating partial slots) and each CTA of the exch
 the kernel's steps, runs them under a seeded random scheduler and checks the properties above.  The same simulator shows
 that the buffer counts the kernels rely on are necessary: ONE partial slot breaks the one-shot protocol (it has no trailing
 barrier), while the two-shot protocol (barrier B) is safe even then, and a single x_out buffer suffices.
-It validates the design the kernels implement - not the CUDA code itself (that is tests/test_tp_gpu.py)."""
+It validates the design the kernels implement - not the CUDA code itself (tests/test_exchange_kernels_gpu.py holds the kernels
+to a bit-exact restatement on one GPU, tests/test_tp_gpu.py runs them across GPUs)."""
 import random
 
 import pytest

@@ -6,11 +6,14 @@ data.  What must hold for every interleaving of ranks and CTAs and every deliver
   * a pushed unit never overwrites a line its receiver has not consumed yet (receive buffers are reused every second exchange:
     slot = k % 2),
   * the GEMM that follows sees every row of x_out from this exchange,
-  * nobody waits forever - PROVIDED every CTA of the grid is resident (the kernel caps its grid at 2 CTAs per SM for that reason;
-    the simulator shows the cap is necessary).
+  * nobody waits forever - PROVIDED every CTA can eventually run alongside the peer CTAs it waits for.  The simulator dispatches
+    CTAs in any order, so it needs the whole grid resident and shows why.  The kernel's grid of 2 CTAs per SM is not always one
+    wave (at 512 threads one CTA fits per SM); it relies on CTA c waiting only for CTA c of each peer and on CTAs being
+    dispatched in blockIdx order (csrc/allreduce_ll.cu).
 The model: per rank a stream (GEMM -> exchange kernel -> consumer GEMM), per CTA a state machine that mirrors the kernel's three
 phases, a network that delivers every pushed half-line independently after an arbitrary delay and in arbitrary order, all under
-a seeded random scheduler.  It validates the protocol the kernel implements, not the CUDA code (tests/test_tp_gpu.py does)."""
+a seeded random scheduler.  It validates the protocol the kernel implements, not the CUDA code (tests/test_exchange_kernels_gpu.py
+holds the kernel to a bit-exact restatement on one GPU, tests/test_tp_gpu.py runs it across GPUs)."""
 import random
 
 import pytest
@@ -174,8 +177,9 @@ def test_ll_protocol_with_a_different_row_count_every_exchange():
 
 
 def test_ll_protocol_needs_every_cta_resident():
-    """The simulator has teeth, and documents why the kernel caps its grid: with fewer resident CTAs than launched, the CTAs that
-    wait for a peer's rows can occupy every slot while the CTAs that would push to that peer cannot start."""
+    """The simulator has teeth, and documents why residency matters: with fewer resident CTAs than launched and CTAs dispatched
+    in any order, the CTAs that wait for a peer's rows can occupy every slot while the CTAs that would push to that peer cannot
+    start."""
     dead = 0
     for seed in range(40):
         try:
