@@ -10,6 +10,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --temperature 0.8 --top-p 0.95 [--top-k 50] [--seed 1]    sample instead of greedy decoding
     ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
+    ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
 """
 import argparse
 import os
@@ -23,10 +24,22 @@ import torch  # noqa: E402
 import swiftllm_b200  # noqa: E402
 
 
-def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None):
+def prompt_lookup(tokens: list, k: int, max_ngram: int = 3) -> list:
+    """Up to k draft tokens: what followed the most recent earlier occurrence of the longest suffix n-gram (n <= max_ngram) of
+    `tokens`; none when no suffix recurs."""
+    for n in range(min(max_ngram, len(tokens) - 1), 0, -1):
+        tail = tokens[-n:]
+        for s in range(len(tokens) - n - 1, -1, -1):
+            if tokens[s:s + n] == tail:
+                return tokens[s + n:s + n + k]
+    return []
+
+
+def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0):
     """Generation for a batch of prompts (sequence i uses block-table row i), greedy unless `params` (one
     swiftllm_b200.SamplingParams for every sequence) is given.  chunk > 0: the prompts are prefilled `chunk` tokens at a time
-    through the paged cache.  Returns (token lists, prefill seconds, decode seconds).
+    through the paged cache.  speculate > 0: decoding verifies up to that many prompt-lookup drafts per step
+    (forward_speculative); the tokens are the ones plain decoding returns.  Returns (token lists, prefill seconds, decode seconds).
     With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token."""
     seq_ids = list(range(len(input_ids)))
     sp = (lambda n: None) if params is None else (lambda n: [params] * n)
@@ -59,6 +72,16 @@ def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, log
     outputs = [[t] for t in last]
     seq_lens = [len(p) for p in input_ids]
     t0 = time.perf_counter()
+    if speculate > 0:                  # every call verifies up to `speculate` prompt-lookup drafts per unfinished sequence
+        while any(len(o) < new_tokens for o in outputs):
+            live = [i for i in seq_ids if len(outputs[i]) < new_tokens]
+            entries = [[outputs[i][-1]] + prompt_lookup(input_ids[i] + outputs[i], min(speculate, new_tokens - len(outputs[i]) - 1))
+                       for i in live]
+            res = model.forward_speculative(entries, live, [seq_lens[i] for i in live], sampling_params_list=sp(len(live)))
+            for i, r in zip(live, res):
+                outputs[i] += r
+                seq_lens[i] += len(r)
+        return outputs, t_prefill, time.perf_counter() - t0
     for _ in range(new_tokens - 1):
         seq_lens = [n + 1 for n in seq_lens]
         last = step([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(len(seq_ids)))
@@ -88,7 +111,13 @@ def main():
     ap.add_argument("--repetition-penalty", type=float, default=1.0, help="divide / multiply the logits of seen tokens (1 = off)")
     ap.add_argument("--frequency-penalty", type=float, default=0.0, help="subtract this times each token's output count (0 = off)")
     ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
+    ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
     args = ap.parse_args()
+    if not 0 <= args.speculate <= 7:
+        ap.error("--speculate takes 0..7 drafts")
+    if args.speculate and (args.logprobs is not None or args.repetition_penalty != 1.0 or args.frequency_penalty != 0.0
+                           or args.presence_penalty != 0.0):
+        ap.error("--speculate does not combine with --logprobs or penalties")
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
                                     num_cpu_blocks=0, max_seqs_in_block_table=128, max_blocks_per_seq=2048, max_batch_size=16,
@@ -122,7 +151,7 @@ def main():
     if args.temperature == 0 and args.logprobs is None and not params.has_penalties():
         params = None
     logs = [[] for _ in input_ids]
-    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs)
+    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs, args.speculate)
     seq_ids = list(range(len(input_ids)))
     for p, o, lg in zip(input_ids, outputs, logs):
         print(f"[{len(p)} prompt tokens] -> {show(o)}")

@@ -130,6 +130,23 @@ int sllm_prefill_attention_paged(const void* q, const void* k_cache, const void*
                                  int max_blocks_per_seq, int64_t num_blocks, int64_t q_row_stride, sllm_dtype_t dtype,
                                  sllm_stream_t stream);
 
+/* ---- Speculative verification (new): the function of sllm_prefill_attention_paged for entries of 1..8 query rows.
+ * Entry i has row_counts[i] <= max_rows rows starting at q / o row start_locs[i]; row j sits at position prefix_lens[i] + j
+ * (its K/V stored first) and attends to positions 0 .. prefix_lens[i] + j through rows `seq_ids` of the block table.  The
+ * entries' rows must tile o's rows [0, num_tokens); max_seq_len >= max_i(prefix_lens[i] + row_counts[i]).  head_dim 128,
+ * block_size 16 and (nq / nkv) * max_rows <= 32 run the sm_90a multi-query kernel: one work item per (entry, kv head,
+ * split) reads each K/V page once for all the entry's rows and heads, splits as in sllm_paged_attention (over entries x kv
+ * heads) merged per row.  Other shapes run sllm_prefill_attention_paged.  workspace: at least
+ * sllm_paged_attention_verify_workspace_bytes(...) bytes of device memory (may be NULL when that is 0). */
+int64_t sllm_paged_attention_verify_workspace_bytes(int num_seqs, int64_t num_tokens, int num_q_heads, int num_kv_heads,
+                                                    int head_dim, int max_seq_len);
+int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* v_cache, void* o, const int32_t* block_table,
+                                const int32_t* seq_ids, const int32_t* start_locs, const int32_t* row_counts,
+                                const int32_t* prefix_lens, void* workspace, int64_t workspace_bytes, float softmax_scale,
+                                int num_seqs, int max_rows, int max_seq_len, int64_t num_tokens, int cur_layer, int num_layers,
+                                int num_q_heads, int num_kv_heads, int block_size, int head_dim, int max_blocks_per_seq,
+                                int64_t num_blocks, int64_t q_row_stride, sllm_dtype_t dtype, sllm_stream_t stream);
+
 /* ---- Block-table maintenance: swiftllm/worker/kernels/block_mgmt.py:26-46, :66-80, :106-127
  * block_table int32 [max_seqs, max_blocks_per_seq]; num_seq_allocated_blocks int32 [max_seqs];
  * is_block_free uint8/bool [num_blocks]; candidate_blocks int64 [sum(block_needed)];
@@ -147,6 +164,12 @@ int sllm_gather_allocated_blocks_and_unset(int32_t* num_seq_allocated_blocks, co
                                            const int32_t* seq_ids, uint8_t* is_block_free,
                                            const int32_t* allocated_cumsum, int32_t* gathered_block_ids,
                                            int batch_size, int max_blocks_per_seq, sllm_stream_t stream);
+/* Shrink sequence seq_ids[i] to cdiv(target_lens[i], block_size) blocks (new; speculative steps give back blocks that only
+ * held rejected drafts): table entries [cdiv(target, block_size), num_seq_allocated_blocks) are marked free and the count is
+ * lowered.  A target at or above the current allocation changes nothing.  seq_ids must be distinct. */
+int sllm_truncate_blocks_for_seqs(int32_t* num_seq_allocated_blocks, const int32_t* block_table, uint8_t* is_block_free,
+                                  const int32_t* seq_ids, const int32_t* target_lens, int batch_size, int block_size,
+                                  int max_blocks_per_seq, sllm_stream_t stream);
 
 /* ---- Sync-free block allocation (replaces swiftllm/worker/block_manager.py:43-79: assert + .item() +
  * torch.nonzero).  One launch: for seq i (batch order) needs max(0, cdiv(target_lens[i], block_size) -

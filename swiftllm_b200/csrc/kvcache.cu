@@ -109,6 +109,21 @@ __global__ void unset_block_table_kernel(int32_t* nsab, const int32_t* block_tab
     if (lane == 0) nsab[sid] = 0;
 }
 
+// Give back the blocks past ceil(target_lens[b] / bs) of each sequence (speculative steps: blocks that only held rejected
+// drafts).  One warp per sequence; a target at or above the allocation changes nothing.
+__global__ void truncate_blocks_kernel(int32_t* __restrict__ nsab, const int32_t* __restrict__ block_table,
+                                       uint8_t* __restrict__ is_free, const int32_t* __restrict__ seq_ids,
+                                       const int32_t* __restrict__ target_lens, int batch, int bs, int mbps) {
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    const int64_t sid = seq_ids[b];
+    const int n = nsab[sid];
+    const int keep = min(n, (target_lens[b] + bs - 1) / bs);
+    for (int i = keep + lane; i < n; i += 32) is_free[block_table[sid * mbps + i]] = 1;
+    __syncwarp();
+    if (lane == 0) nsab[sid] = keep;
+}
+
 // ------------------------------------------------------------------ sync-free allocation
 // Replaces block_manager.py:43-79 (assert(...).all() + sum().item() + torch.nonzero()[:n]) by one launch of a
 // single CTA.  Ordering contract (bit-exact block ids): the n lowest-numbered free blocks, ascending, are
@@ -336,6 +351,16 @@ int sllm_gather_allocated_blocks_and_unset(int32_t* nsab, const int32_t* block_t
     unset_block_table_kernel<true><<<cdiv(batch, 4), 128, 0, (cudaStream_t)stream>>>(nsab, block_table, seq_ids, is_free,
                                                                                       cumsum, gathered, batch, mbps);
     return check_launch("gather_allocated_blocks_and_unset");
+}
+
+int sllm_truncate_blocks_for_seqs(int32_t* nsab, const int32_t* block_table, uint8_t* is_free, const int32_t* seq_ids,
+                                  const int32_t* target_lens, int batch, int block_size, int mbps, sllm_stream_t stream) {
+    SLLM_REQUIRE(batch >= 0 && block_size > 0 && mbps > 0, "truncate_blocks: bad sizes");
+    if (batch == 0) return 0;
+    SLLM_REQUIRE(nsab && block_table && is_free && seq_ids && target_lens, "truncate_blocks: null pointer");
+    truncate_blocks_kernel<<<cdiv(batch, 4), 128, 0, (cudaStream_t)stream>>>(nsab, block_table, is_free, seq_ids, target_lens,
+                                                                             batch, block_size, mbps);
+    return check_launch("truncate_blocks_for_seqs");
 }
 
 int sllm_allocate_blocks_for_seqs(int32_t* nsab, int32_t* block_table, uint8_t* is_free, const int32_t* seq_ids,

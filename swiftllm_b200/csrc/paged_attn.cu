@@ -278,6 +278,14 @@ int launch_paged_tc(const void* q, const void* k_cache, const void* v_cache, con
                     const int32_t* seq_lens, void* o, float* part_o, float* part_lse, float scale_log2e, int num_seqs,
                     int split_tokens, int num_splits, int cur_layer, int num_layers, int nq, int nkv, int max_blocks_per_seq,
                     int64_t num_blocks, int64_t q_row_stride, sllm_dtype_t dtype, int num_sms, cudaStream_t stream);
+bool tc_verify_supported(int head_dim, int block_size, int nq, int nkv, int max_rows, int64_t num_blocks, int num_layers,
+                         int64_t num_tokens);
+int launch_paged_verify_tc(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table,
+                           const int32_t* seq_ids, const int32_t* start_locs, const int32_t* row_counts,
+                           const int32_t* prefix_lens, void* o, float* part_o, float* part_lse, int32_t* row_lens,
+                           float scale_log2e, int num_seqs, int max_rows, int64_t num_tokens, int split_tokens, int num_splits,
+                           int cur_layer, int num_layers, int nq, int nkv, int max_blocks_per_seq, int64_t num_blocks,
+                           int64_t q_row_stride, sllm_dtype_t dtype, int num_sms, cudaStream_t stream);
 
 // SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements, debugging); default: TMA/wgmma
 // whenever the shape is covered (head_dim 128, block_size 16).
@@ -372,6 +380,67 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
     if (head_dim == 128) { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 128>(p, num_decoding_seqs, max_seq_len, st))); }
     else { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 64>(p, num_decoding_seqs, max_seq_len, st))); }
     return 0;
+}
+
+// ---- speculative verification: splits are planned over (entries x kv heads) with the longest visible length, partials are
+// [rows, nq, num_splits] + per-row visible lengths (int32 [num_tokens]), merged by paged_attn_merge_kernel
+int64_t sllm_paged_attention_verify_workspace_bytes(int num_seqs, int64_t num_tokens, int nq, int nkv, int head_dim,
+                                                    int max_seq_len) {
+    if (num_seqs <= 0 || num_tokens <= 0 || max_seq_len <= 0 || nkv <= 0) return 0;
+    const int st = choose_split_tokens(num_seqs, nkv, max_seq_len, 0);
+    const int64_t ns = (max_seq_len + st - 1) / st;
+    if (ns <= 1) return 0;
+    return num_tokens * nq * ns * (head_dim + 1) * (int64_t)sizeof(float) + num_tokens * (int64_t)sizeof(int32_t);
+}
+
+int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* v_cache, void* o, const int32_t* block_table,
+                                const int32_t* seq_ids, const int32_t* start_locs, const int32_t* row_counts,
+                                const int32_t* prefix_lens, void* workspace, int64_t workspace_bytes, float softmax_scale,
+                                int num_seqs, int max_rows, int max_seq_len, int64_t num_tokens, int cur_layer, int num_layers,
+                                int nq, int nkv, int block_size, int head_dim, int max_blocks_per_seq, int64_t num_blocks,
+                                int64_t q_row_stride, sllm_dtype_t dtype, sllm_stream_t stream) {
+    SLLM_REQUIRE(num_seqs >= 0 && num_tokens >= 0, "paged_attention_verify: negative sizes");
+    if (num_seqs == 0) return 0;
+    SLLM_REQUIRE(q && k_cache && v_cache && o && block_table && seq_ids && start_locs && row_counts && prefix_lens,
+                 "paged_attention_verify: null pointer");
+    SLLM_REQUIRE(max_rows >= 1 && max_rows <= 8, "paged_attention_verify: max_rows %d outside [1, 8]", max_rows);
+    SLLM_REQUIRE(num_tokens >= max_rows && max_seq_len >= max_rows, "paged_attention_verify: num_tokens / max_seq_len below max_rows");
+    SLLM_REQUIRE(head_dim == 64 || head_dim == 128, "paged_attention_verify: head_dim %d not supported (64, 128)", head_dim);
+    SLLM_REQUIRE(nkv > 0 && nq % nkv == 0, "paged_attention_verify: nq %d not a multiple of nkv %d", nq, nkv);
+    SLLM_REQUIRE(q_row_stride >= (int64_t)nq * head_dim && q_row_stride % 8 == 0, "paged_attention_verify: bad q row stride");
+    SLLM_REQUIRE(block_size > 0 && num_layers > 0 && cur_layer >= 0 && cur_layer < num_layers && max_blocks_per_seq > 0 && num_blocks > 0,
+                 "paged_attention_verify: bad cache geometry (layer %d of %d)", cur_layer, num_layers);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype <= SLLM_BF16 && tc_verify_supported(head_dim, block_size, nq, nkv, max_rows, num_blocks, num_layers, num_tokens)) {
+        const int split_tokens = choose_split_tokens(num_seqs, nkv, max_seq_len, 0);
+        const int num_splits = (max_seq_len + split_tokens - 1) / split_tokens;
+        float *part_o = nullptr, *part_lse = nullptr;
+        int32_t* row_lens = nullptr;
+        if (num_splits > 1) {
+            const int64_t need = sllm_paged_attention_verify_workspace_bytes(num_seqs, num_tokens, nq, nkv, head_dim, max_seq_len);
+            SLLM_REQUIRE(workspace && workspace_bytes >= need, "paged_attention_verify: workspace too small (%lld < %lld bytes)",
+                         (long long)workspace_bytes, (long long)need);
+            part_o = (float*)workspace;
+            part_lse = part_o + num_tokens * nq * num_splits * head_dim;
+            row_lens = (int32_t*)(part_lse + num_tokens * nq * num_splits);
+        }
+        int e = launch_paged_verify_tc(q, k_cache, v_cache, block_table, seq_ids, start_locs, row_counts, prefix_lens, o, part_o,
+                                       part_lse, row_lens, softmax_scale * 1.4426950408889634f, num_seqs, max_rows, num_tokens,
+                                       split_tokens, num_splits, cur_layer, num_layers, nq, nkv, max_blocks_per_seq, num_blocks,
+                                       q_row_stride, dtype, num_sms(), st);
+        if (e) return e;
+        if (num_splits > 1) {
+            dim3 g2(nq, (unsigned)num_tokens);
+            SLLM_DISPATCH_DTYPE(dtype, (paged_attn_merge_kernel<T><<<g2, head_dim, 0, st>>>(part_o, part_lse, (T*)o, row_lens, nq,
+                                                                                          head_dim, num_splits, split_tokens)));
+            return check_launch("paged_attention_verify(merge)");
+        }
+        return 0;
+    }
+    // shapes the verify kernel does not serve: the chunked-prefill kernel computes the same function (rows = chunk tokens)
+    return sllm_prefill_attention_paged(q, k_cache, v_cache, o, block_table, seq_ids, start_locs, row_counts, prefix_lens,
+                                        softmax_scale, num_seqs, max_rows, num_tokens, cur_layer, num_layers, nq, nkv, block_size,
+                                        head_dim, max_blocks_per_seq, num_blocks, q_row_stride, dtype, stream);
 }
 
 }  // extern "C"

@@ -11,6 +11,7 @@ import torch
 
 from .kernels.block_mgmt import (allocate_blocks_for_seqs as _allocate_kernel,
                                  gather_allocated_blocks_and_unset,
+                                 truncate_blocks_for_seqs as _truncate_kernel,
                                  unset_block_table_and_num_seq_alloc_blocks)
 
 
@@ -68,6 +69,27 @@ class BlockManager:
             self._host_nsab[idx] = target
             self.num_free_blocks -= total
         return new_blocks
+
+    def truncate_blocks_for_seqs(self, seq_ids: torch.Tensor, target_lens: torch.Tensor, *, seq_ids_list=None,
+                                 target_lens_list=None):
+        """Shrink seq #i to ceil(target_lens[i] / block_size) blocks; the blocks past it become free (and are handed out again
+        lowest id first).  A target above the current allocation is a logic error.  Pass the host lists to avoid a sync."""
+        sids = self._to_list(seq_ids, seq_ids_list)
+        lens = self._to_list(target_lens, target_lens_list)
+        if not sids:
+            return
+        idx = np.asarray(sids, dtype=np.int64)
+        target = (np.asarray(lens, dtype=np.int64) + (self.block_size - 1)) // self.block_size
+        have = self._host_nsab[idx]
+        assert (target <= have).all(), \
+            f"(On {self.device_name}) Logic error: truncating sequences to more blocks than they hold."
+        total = int((have - target).sum())
+        if total == 0:
+            return
+        _truncate_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free,
+                         seq_ids.to(torch.int32).contiguous(), target_lens.to(torch.int32).contiguous(), self.block_size)
+        self._host_nsab[idx] = target
+        self.num_free_blocks += total
 
     def check_device_status(self):
         """Debug/test helper (syncs): the allocator kernel's own error flag."""

@@ -49,6 +49,9 @@ class LlamaInferState:
     # the KV cache.  None = whole prompts, attention over the packed k/v.
     prefill_prefix_lens: Optional[torch.Tensor] = None  # [num_prefill_seqs]
     max_prefill_kv_len: int = 0                          # max_i(prefix_i + chunk_i); 0 when not chunked
+    # Speculative verification (LlamaModel.forward_speculative): the chunks are an input token plus drafts (1..8 rows), attended
+    # by the multi-query verify kernel instead of the chunked-prefill kernel
+    speculative: bool = False
     # Per-row sampling parameters (SamplingParams) on the device; None = greedy argmax for every row
     sampling: Optional["SamplingState"] = None
     # Top-N of the step's log-probabilities (the largest SamplingParams.logprobs of the batch); None = no log-probabilities,

@@ -56,6 +56,22 @@ def gather_allocated_blocks_and_unset(
     return gathered
 
 
+def truncate_blocks_for_seqs(
+    num_seq_allocated_blocks: torch.Tensor,
+    block_table: torch.Tensor,
+    is_block_free: torch.Tensor,
+    seq_ids: torch.Tensor,                   # [batch] int32, distinct
+    target_lens: torch.Tensor,               # [batch] int32
+    block_size: int,
+):
+    """Free the blocks past ceil(target_lens[i] / block_size) of every sequence (one launch, no host sync)."""
+    _lib.require_device(block_table)
+    assert seq_ids.dtype == torch.int32 and target_lens.dtype == torch.int32 and is_block_free.dtype == torch.bool
+    _lib.check(_lib.lib().sllm_truncate_blocks_for_seqs(
+        num_seq_allocated_blocks.data_ptr(), block_table.data_ptr(), is_block_free.data_ptr(), seq_ids.data_ptr(),
+        target_lens.data_ptr(), seq_ids.shape[0], block_size, block_table.shape[1], _lib.stream()), "truncate_blocks_for_seqs")
+
+
 def allocate_blocks_for_seqs(
     num_seq_allocated_blocks: torch.Tensor,
     block_table: torch.Tensor,

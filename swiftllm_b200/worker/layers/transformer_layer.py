@@ -15,7 +15,7 @@ from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.kvcache_mgmt import rotary_store_kvcache_decode, store_kvcache
 from swiftllm_b200.worker.kernels.linear import linear
 from swiftllm_b200.worker.kernels.paged_attn import paged_attention
-from swiftllm_b200.worker.kernels.prefill_attn import prefill_attention, prefill_attention_paged
+from swiftllm_b200.worker.kernels.prefill_attn import paged_attention_verify, prefill_attention, prefill_attention_paged
 from swiftllm_b200.worker.kernels.rmsnorm import fused_add_rmsnorm_inplace
 from swiftllm_b200.worker.kernels.rotary_emb import rotary_embedding_inplace
 from swiftllm_b200.worker.kernels.silu_and_mul import silu_and_mul_inplace
@@ -85,9 +85,9 @@ class LlamaTransformerLayer:
         if infer_state.num_prefill_seqs > 0:
             if infer_state.prefill_prefix_lens is not None:
                 # chunked prefill: attend to prefix + chunk through the block table (the chunk's K/V were stored above)
-                prefill_attention_paged(q[:npt], k_cache, v_cache, block_table,
-                                        o[:npt].view(npt, self.num_q_heads, mc.head_dim), mc, self.engine_config,
-                                        infer_state, self.layer_id)
+                attend = paged_attention_verify if infer_state.speculative else prefill_attention_paged
+                attend(q[:npt], k_cache, v_cache, block_table, o[:npt].view(npt, self.num_q_heads, mc.head_dim), mc,
+                       self.engine_config, infer_state, self.layer_id)
             else:
                 prefill_attention(q[:npt], k[:npt], v[:npt], o[:npt].view(npt, self.num_q_heads, mc.head_dim),
                                   mc, self.engine_config, infer_state)

@@ -4,6 +4,8 @@
     LlamaModel(engine_config) -> load_weights() -> profile_num_blocks() -> init_kvcache_and_swap(num_blocks)
     forward(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False) -> list[int]
     forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities)
+    forward_speculative(input_ids_list, seq_ids_list, prefix_lens_list, sampling_params_list=None) -> list[list[int]]
+                                                            (addition: verify up to 7 drafts per sequence in one step)
     swap_in_seqs / swap_out_seqs / free_seqs_resources
 
 and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).  Addition: the token
@@ -355,6 +357,91 @@ class LlamaModel:
                 n = min(int(n), self.model_config.vocab_size)
                 res.append(TokenLogprobs(t, token_lp[i], list(zip(top_ids[i][:n], top_lp[i][:n]))))
         return res
+
+    MAX_SPECULATIVE_ROWS = 8
+
+    @torch.inference_mode()
+    def forward_speculative(self, input_ids_list: list, seq_ids_list: list, prefix_lens_list: list,
+                            sampling_params_list: Optional[list] = None, ignore_kvcache: bool = False) -> list:
+        """Speculative decoding: score a plain decode input and up to 7 caller-made drafts per sequence in one step.
+
+        Entry i is input_ids_list[i] = [x, d_1, ..., d_k] (1 <= k + 1 <= 8): x is the token a plain decode step would feed, d_* are
+        drafts (prompt lookup, an n-gram table, another model's greedy output).  prefix_lens_list[i] tokens of the sequence are in
+        the KV cache (decoding_seq_len - 1 of the equivalent forward() step); row j sits at position prefix_i + j.  For every row
+        j, y_j is the token forward() would return for a decode step at that position: argmax, or the sampling kernel with the
+        entry's SamplingParams (one seed for all the entry's rows) and pos = prefix_i + j + 1.  With n the number of leading
+        drafts such that d_{j+1} == y_j, entry i returns [y_0, ..., y_n]: exactly the tokens n + 1 plain steps would return.
+
+        Afterwards the sequence has prefix_i + 1 + n cached tokens and holds ceil((prefix_i + 1 + n) / block_size) blocks: continue
+        it with forward() at decoding_seq_len prefix_i + n + 2 and input y_n, or with forward_speculative at prefix prefix_i + 1 + n.
+        K/V of rejected rows inside a kept block are overwritten by later steps (attention never reads past a row's position).
+        Speculative entries only (no prompts in the same call); runs eagerly and syncs once, like forward().  Raises ValueError
+        before anything is enqueued for: a row count outside [1, 8], a negative prefix or one whose rows run past the position
+        table, ignore_kvcache, invalid sampling parameters, and penalties.  SamplingParams.logprobs is ignored."""
+        B = len(input_ids_list)
+        if len(seq_ids_list) != B or len(prefix_lens_list) != B:
+            raise ValueError(f"forward_speculative: {B} entries but {len(seq_ids_list)} seq ids and {len(prefix_lens_list)} prefixes")
+        if ignore_kvcache:
+            raise ValueError("forward_speculative reads and writes the KV cache: ignore_kvcache is not applicable")
+        rows = [len(x) for x in input_ids_list]
+        prefix = [int(p) for p in prefix_lens_list]
+        max_pos = self._cos_cached.shape[0]
+        for n, p in zip(rows, prefix):
+            if not 1 <= n <= self.MAX_SPECULATIVE_ROWS:
+                raise ValueError(f"forward_speculative: an entry has {n} rows; 1 to {self.MAX_SPECULATIVE_ROWS} are supported")
+            if p < 0 or p + n > max_pos:
+                raise ValueError(f"forward_speculative: prefix {p} with {n} rows is outside the position table [0, {max_pos})")
+        samp = None if sampling_params_list is None else sampling_words(sampling_params_list, B, self._sampling_rng)
+        if has_penalties(sampling_params_list):
+            raise ValueError("forward_speculative does not apply penalties (their history is per position)")
+        if B == 0:
+            return []
+        mc = self.model_config
+        T = sum(rows)
+        rep = np.repeat(np.arange(B), rows)
+        flat_ids = list(itertools.chain(*input_ids_list))
+        starts = list(itertools.accumulate([0] + rows[:-1]))
+        positions = [p + j for p, n in zip(prefix, rows) for j in range(n)]
+        seq_lengths = [p + n for p, n in zip(prefix, rows)]
+        row_pos = [q + 1 for q in positions]             # sampling noise counter of row j: prefix + j + 1
+        if samp is not None:
+            # the words are per entry: every row of an entry gets its parameters and its seed
+            w = np.asarray(samp[0], dtype=np.int64)
+            row_words = np.concatenate([w[:2 * B].reshape(B, 2)[rep].reshape(-1)] +
+                                       [w[(2 + s) * B:(3 + s) * B][rep] for s in range(3)]).tolist()
+        views = self._stage_metadata(*([row_words] if samp else []), flat_ids, seq_ids_list, seq_lengths, rows, starts,
+                                     positions, range(T), prefix, row_pos)
+        ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, p_prefix, r_pos = views[-9:]
+        sampling = SamplingState.from_staged(views[0], r_pos, samp[1]) if samp else None
+        bm = self.gpu_block_manager
+        bm.allocate_blocks_for_seqs(seq_ids, seq_lens, seq_ids_list=seq_ids_list, target_lens_list=seq_lengths,
+                                    want_new_blocks=False)
+        infer_state = LlamaInferState(
+            batch_size=B, num_tokens=T, seq_ids=seq_ids, softmax_scale=mc.head_dim ** -0.5,
+            num_prefill_seqs=B, num_prefill_tokens=T, prefill_seq_start_locs=p_starts,
+            prefill_seq_start_locs_with_end=torch.cat([p_starts, p_starts.new_tensor([T])]),
+            prefill_seq_lens=p_lens, max_prefill_len=max(rows),
+            num_decoding_seqs=0, decoding_seq_lens=seq_lens[B:], max_decoding_len=0,
+            seq_block_size=select_seq_block_size(mc.num_kv_heads, [], 0), num_seq_blocks=0,
+            position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
+            ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last,
+            prefill_prefix_lens=p_prefix, max_prefill_kv_len=max(seq_lengths), sampling=sampling, speculative=True,
+        )
+        tokens = self._forward(ids, infer_state).tolist()
+        out, keep = [], []
+        for ids_i, s, n_rows, p in zip(input_ids_list, starts, rows, prefix):
+            y = tokens[s:s + n_rows]
+            n = 0
+            while n < n_rows - 1 and int(ids_i[n + 1]) == y[n]:
+                n += 1
+            out.append(y[:n + 1])
+            keep.append(p + 1 + n)
+        # give back the blocks that only held rejected rows
+        bs = bm.block_size
+        if any((k + bs - 1) // bs < (L + bs - 1) // bs for k, L in zip(keep, seq_lengths)):
+            bm.truncate_blocks_for_seqs(seq_ids, torch.tensor(keep, dtype=torch.int32, device=self.device),
+                                        seq_ids_list=seq_ids_list, target_lens_list=keep)
+        return out
 
     def _step(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
               sampling_params_list, with_logprobs: bool):
