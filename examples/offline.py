@@ -11,8 +11,10 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
+    ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
 """
 import argparse
+import dataclasses
 import os
 import sys
 import time
@@ -35,16 +37,27 @@ def prompt_lookup(tokens: list, k: int, max_ngram: int = 3) -> list:
     return []
 
 
-def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0):
+def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0, n: int = 1):
     """Generation for a batch of prompts (sequence i uses block-table row i), greedy unless `params` (one
     swiftllm_b200.SamplingParams for every sequence) is given.  chunk > 0: the prompts are prefilled `chunk` tokens at a time
     through the paged cache.  speculate > 0: decoding verifies up to that many prompt-lookup drafts per step
     (forward_speculative); the tokens are the ones plain decoding returns.  Returns (token lists, prefill seconds, decode seconds).
-    With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token."""
-    seq_ids = list(range(len(input_ids)))
-    sp = (lambda n: None) if params is None else (lambda n: [params] * n)
+    With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token.
+
+    n > 1: n samples per prompt.  Each prompt is prefilled once into row i; rows len(input_ids) + i * (n - 1) + j (j < n - 1)
+    fork its first len - 1 tokens (fork_seqs: the full blocks are shared) and draw their own first token from the last prompt
+    token, fed as a one-token prefill chunk so that penalties count it as a prompt token, as in row i.  Sample k of a prompt uses seed params.seed + k (seed None: a fresh seed per row and step), so the samples differ; the
+    n * len(input_ids) sequences then decode in one batch.  Outputs and logs follow the rows: prompts first, then the forks."""
+    P = len(input_ids)
+    seq_ids = list(range(P))
+    kids = [(i, P + i * (n - 1) + j, j + 1) for i in range(P) for j in range(n - 1)]     # (prompt, row, sample index)
+    if kids and min(len(p) for p in input_ids) < 2:
+        raise ValueError("n > 1 forks len - 1 prompt tokens: every prompt needs at least 2 tokens")
+    row_params = [params] * P + [params if params is None or params.seed is None else
+                                 dataclasses.replace(params, seed=(params.seed + k) % 2 ** 64) for _, _, k in kids]
+    sp = (lambda rows: None) if params is None else (lambda rows: [row_params[i] for i in rows])
     want_lp = params is not None and params.logprobs is not None
-    logs = logs if logs is not None else [[] for _ in input_ids]
+    logs = logs if logs is not None else [[] for _ in range(P * n)]
 
     def step(*args, **kw):
         if not want_lp:
@@ -57,13 +70,21 @@ def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, log
         while any(d < len(p) for d, p in zip(done, input_ids)):
             live = [i for i in seq_ids if done[i] < len(input_ids[i])]
             toks = step([input_ids[i][done[i]:done[i] + chunk] for i in live], live, [],
-                        prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(len(live)))
+                        prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(live))
             for i, t in zip(live, toks):
                 done[i] = min(len(input_ids[i]), done[i] + chunk)
                 if done[i] == len(input_ids[i]):
                     last[i] = t             # the token sampled after the LAST chunk is the first generated token
     else:
-        last = step(input_ids, seq_ids, [], sampling_params_list=sp(len(seq_ids)))
+        last = step(input_ids, seq_ids, [], sampling_params_list=sp(seq_ids))
+    if kids:
+        rows = [r for _, r, _ in kids]
+        model.fork_seqs([i for i, _, _ in kids], rows, [len(input_ids[i]) - 1 for i, _, _ in kids])
+        last = list(last) + list(step([[input_ids[i][-1]] for i, _, _ in kids], rows, [],
+                                      prefill_prefix_lens_list=[len(input_ids[i]) - 1 for i, _, _ in kids],
+                                      sampling_params_list=sp(rows)))
+        input_ids = list(input_ids) + [input_ids[i] for i, _, _ in kids]
+        seq_ids = seq_ids + rows
     if want_lp:
         for lg, r in zip(logs, last):
             lg.append(r)
@@ -77,14 +98,14 @@ def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, log
             live = [i for i in seq_ids if len(outputs[i]) < new_tokens]
             entries = [[outputs[i][-1]] + prompt_lookup(input_ids[i] + outputs[i], min(speculate, new_tokens - len(outputs[i]) - 1))
                        for i in live]
-            res = model.forward_speculative(entries, live, [seq_lens[i] for i in live], sampling_params_list=sp(len(live)))
+            res = model.forward_speculative(entries, live, [seq_lens[i] for i in live], sampling_params_list=sp(live))
             for i, r in zip(live, res):
                 outputs[i] += r
                 seq_lens[i] += len(r)
         return outputs, t_prefill, time.perf_counter() - t0
     for _ in range(new_tokens - 1):
         seq_lens = [n + 1 for n in seq_lens]
-        last = step([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(len(seq_ids)))
+        last = step([[t] for t in last], seq_ids, seq_lens, sampling_params_list=sp(seq_ids))
         if want_lp:
             for lg, r in zip(logs, last):
                 lg.append(r)
@@ -112,7 +133,10 @@ def main():
     ap.add_argument("--frequency-penalty", type=float, default=0.0, help="subtract this times each token's output count (0 = off)")
     ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
     ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
+    ap.add_argument("--n", type=int, default=1, help="samples per prompt: prefill once, fork n - 1 times, distinct seeds (1 = off)")
     args = ap.parse_args()
+    if args.n < 1:
+        ap.error("--n takes a positive number of samples")
     if not 0 <= args.speculate <= 7:
         ap.error("--speculate takes 0..7 drafts")
     if args.speculate and (args.logprobs is not None or args.repetition_penalty != 1.0 or args.frequency_penalty != 0.0
@@ -150,10 +174,13 @@ def main():
                                           presence_penalty=args.presence_penalty)
     if args.temperature == 0 and args.logprobs is None and not params.has_penalties():
         params = None
-    logs = [[] for _ in input_ids]
-    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs, args.speculate)
-    seq_ids = list(range(len(input_ids)))
-    for p, o, lg in zip(input_ids, outputs, logs):
+    logs = [[] for _ in range(len(input_ids) * args.n)]
+    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs, args.speculate, args.n)
+    seq_ids = list(range(len(outputs)))
+    # rows of prompt i: i, then its forks
+    rows = [k for i in range(len(input_ids)) for k in [i] + [len(input_ids) + i * (args.n - 1) + j for j in range(args.n - 1)]]
+    for k in rows:
+        p, o, lg = input_ids[k if k < len(input_ids) else (k - len(input_ids)) // (args.n - 1)], outputs[k], logs[k]
         print(f"[{len(p)} prompt tokens] -> {show(o)}")
         for r in lg:      # log-probabilities of the raw model distribution (before penalties, temperature / top-k / top-p)
             top = ", ".join(f"{show([t])!r}:{lp:.3f}" for t, lp in r.top)

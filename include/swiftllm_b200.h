@@ -184,6 +184,32 @@ int sllm_allocate_blocks_for_seqs(int32_t* num_seq_allocated_blocks, int32_t* bl
                                   int64_t* new_blocks_out, int64_t new_blocks_capacity, int32_t* status_out,
                                   sllm_stream_t stream);
 
+/* ---- Shared blocks (new; fork a cached prefix into another sequence).  block_extra_refs int32 [num_blocks]: owners of a block
+ * beyond the first, 0 for every free and every freshly allocated block (the allocator above reads only is_block_free).
+ * Shared blocks are always the leading blocks of a row.  All three are one launch each, stream-ordered, no host sync.
+ *
+ * Fork: for every entry i, dst_seq_ids[i]'s row gets the first lens[i] / block_size table entries of src_seq_ids[i]'s row,
+ * num_seq_allocated_blocks[dst] is set to that count and each shared block gains one extra owner.  Several entries may name the
+ * same src.  The dst rows must be empty; a partial tail block (lens[i] % block_size != 0) is added by a following
+ * sllm_allocate_blocks_for_seqs with target lens[i], then filled by sllm_copy_block_tails. */
+int sllm_fork_blocks_for_seqs(int32_t* num_seq_allocated_blocks, int32_t* block_table, int32_t* block_extra_refs,
+                              const int32_t* src_seq_ids, const int32_t* dst_seq_ids, const int32_t* lens, int batch_size,
+                              int block_size, int max_blocks_per_seq, sllm_stream_t stream);
+/* For every entry with lens[i] % block_size != 0: copy block lens[i] / block_size of src's row into the same block index of dst's
+ * row, ids read from block_table on the device.  Copies block_bytes bytes of k_cache and of v_cache (one block of every layer:
+ * [num_blocks][block_bytes] with block_bytes a multiple of 16) and, when token_cache (int32 [num_blocks, block_size]) is not NULL,
+ * the block's token page.  batch_size <= 65535. */
+int sllm_copy_block_tails(void* k_cache, void* v_cache, int32_t* token_cache, const int32_t* block_table,
+                          const int32_t* src_seq_ids, const int32_t* dst_seq_ids, const int32_t* lens, int batch_size,
+                          int64_t block_bytes, int block_size, int max_blocks_per_seq, sllm_stream_t stream);
+/* Release every block of the given sequences: a block with extra owners loses one, otherwise it becomes free (several owners
+ * released in one call: exactly one frees it); num_seq_allocated_blocks[seq] becomes 0.  gathered_block_ids may be NULL; when
+ * given, every block id of the sequences is written in batch order as by sllm_gather_allocated_blocks_and_unset
+ * (allocated_cumsum: inclusive cumsum of num_seq_allocated_blocks[seq_ids]). */
+int sllm_release_blocks_for_seqs(int32_t* num_seq_allocated_blocks, const int32_t* block_table, uint8_t* is_block_free,
+                                 int32_t* block_extra_refs, const int32_t* seq_ids, const int32_t* allocated_cumsum,
+                                 int32_t* gathered_block_ids, int batch_size, int max_blocks_per_seq, sllm_stream_t stream);
+
 /* ---- Tensor-parallel exchange fused with the op that follows it (new; the reference is single-GPU):
  *   residual <- h(sum over ranks of partial) + residual ;  x_out <- rmsnorm(residual) * weight
  * i.e. the all-reduce after o_proj / down_proj merged with fused_add_rmsnorm_inplace (rmsnorm.py:67-89) in one kernel that

@@ -42,6 +42,9 @@ SIGNATURES = {
     "sllm_unset_block_table_and_num_seq_alloc_blocks": (_I, [_P, _P, _P, _P, _I, _I, _P]),
     "sllm_gather_allocated_blocks_and_unset": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
     "sllm_allocate_blocks_for_seqs": (_I, [_P, _P, _P, _P, _P, _I, _I, _L, _I, _P, _L, _P, _P]),
+    "sllm_fork_blocks_for_seqs": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "sllm_copy_block_tails": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _L, _I, _I, _P]),
+    "sllm_release_blocks_for_seqs": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _P]),
     "sllm_allreduce_add_rmsnorm": (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _F, _L, _I, _I, _P]),
     "sllm_allreduce_add_rmsnorm_2shot": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _F, _L, _I, _I, _P]),
     "sllm_allreduce_add_rmsnorm_ll": (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _F, _L, _I, _L, _I, _P]),

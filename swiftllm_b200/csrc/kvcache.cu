@@ -124,6 +124,91 @@ __global__ void truncate_blocks_kernel(int32_t* __restrict__ nsab, const int32_t
     if (lane == 0) nsab[sid] = keep;
 }
 
+// ------------------------------------------------------------------ shared blocks (fork)
+// extra_refs[block] = owners beyond the first (0 for every free block and every freshly allocated one), so the allocator,
+// which reads only is_free, needs no change.  Shared blocks are always the leading blocks of a row (a fork shares [0, P / bs)).
+
+// dst_ids[b] takes the first lens[b] / bs blocks of src_ids[b]'s row; one warp per entry.  Several entries may name the same src:
+// the counts are atomic.  The tail block (lens % bs != 0) is appended afterwards by allocate_blocks_kernel.
+__global__ void fork_blocks_kernel(int32_t* __restrict__ nsab, int32_t* __restrict__ block_table, int32_t* __restrict__ extra_refs,
+                                   const int32_t* __restrict__ src_ids, const int32_t* __restrict__ dst_ids,
+                                   const int32_t* __restrict__ lens, int batch, int bs, int mbps) {
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    const int64_t src = src_ids[b], dst = dst_ids[b];
+    const int n = lens[b] / bs;
+    for (int i = lane; i < n; i += 32) {
+        const int32_t id = block_table[src * mbps + i];
+        block_table[dst * mbps + i] = id;
+        atomicAdd(extra_refs + id, 1);
+    }
+    if (lane == 0) nsab[dst] = n;
+}
+
+// Copy block lens[b] / bs of src into the same block index of dst, for every entry with lens[b] % bs != 0: the K and V pages of
+// every layer (one block of all layers is `block_bytes` contiguous bytes, DESIGN §2) and the block's token page.  Both ids are read
+// from the block table.  grid (cdiv(block_bytes, kTailChunk), batch, 2): blockIdx.z picks K or V; each CTA moves one 32 KiB chunk
+// with 8 independent 16-byte loads per thread in flight.
+constexpr int kTailThreads = 256, kTailUnroll = 8, kTailChunk = kTailThreads * kTailUnroll * 16;
+
+__global__ void __launch_bounds__(kTailThreads) copy_block_tails_kernel(
+    char* __restrict__ k_cache, char* __restrict__ v_cache, int32_t* __restrict__ token_cache,
+    const int32_t* __restrict__ block_table, const int32_t* __restrict__ src_ids, const int32_t* __restrict__ dst_ids,
+    const int32_t* __restrict__ lens, int64_t block_bytes, int bs, int mbps) {
+    const int b = blockIdx.y;
+    const int len = lens[b];
+    if (len % bs == 0) return;
+    const int j = len / bs;
+    const int64_t sblk = block_table[(int64_t)src_ids[b] * mbps + j];
+    const int64_t dblk = block_table[(int64_t)dst_ids[b] * mbps + j];
+    char* base = blockIdx.z ? v_cache : k_cache;
+    const uint4* s = reinterpret_cast<const uint4*>(base + sblk * block_bytes);
+    uint4* d = reinterpret_cast<uint4*>(base + dblk * block_bytes);
+    const int64_t nvec = block_bytes >> 4;
+    const int64_t v0 = (int64_t)blockIdx.x * (kTailChunk >> 4) + threadIdx.x;
+    uint4 r[kTailUnroll];
+#pragma unroll
+    for (int u = 0; u < kTailUnroll; u++) {
+        const int64_t v = v0 + u * kTailThreads;
+        if (v < nvec) r[u] = __ldcs(s + v);
+    }
+#pragma unroll
+    for (int u = 0; u < kTailUnroll; u++) {
+        const int64_t v = v0 + u * kTailThreads;
+        if (v < nvec) __stcs(d + v, r[u]);
+    }
+    if (token_cache && blockIdx.x == 0 && blockIdx.z == 0)
+        for (int t = threadIdx.x; t < bs; t += kTailThreads) token_cache[dblk * bs + t] = token_cache[sblk * bs + t];
+}
+
+// Drop one owner of every block of each sequence: a block with extra owners loses one, the releaser that finds none frees it
+// (so of several owners released in one launch exactly one frees the block).  GATHER also writes every block id of the
+// sequences in batch order (the swap plan).  One warp per sequence.
+template <bool GATHER>
+__global__ void release_blocks_kernel(int32_t* __restrict__ nsab, const int32_t* __restrict__ block_table,
+                                      uint8_t* __restrict__ is_free, int32_t* __restrict__ extra_refs,
+                                      const int32_t* __restrict__ seq_ids, const int32_t* __restrict__ cumsum,
+                                      int32_t* __restrict__ gathered, int batch, int mbps) {
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    const int64_t sid = seq_ids[b];
+    const int n = nsab[sid];
+    const int out0 = GATHER ? (b > 0 ? cumsum[b - 1] : 0) : 0;
+    for (int i = lane; i < n; i += 32) {
+        const int32_t id = block_table[sid * mbps + i];
+        if (GATHER) gathered[out0 + i] = id;
+        int old = extra_refs[id];
+        while (old > 0) {
+            const int prev = atomicCAS(extra_refs + id, old, old - 1);
+            if (prev == old) break;
+            old = prev;
+        }
+        if (old == 0) is_free[id] = 1;
+    }
+    __syncwarp();
+    if (lane == 0) nsab[sid] = 0;
+}
+
 // ------------------------------------------------------------------ sync-free allocation
 // Replaces block_manager.py:43-79 (assert(...).all() + sum().item() + torch.nonzero()[:n]) by one launch of a
 // single CTA.  Ordering contract (bit-exact block ids): the n lowest-numbered free blocks, ascending, are
@@ -376,6 +461,47 @@ int sllm_allocate_blocks_for_seqs(int32_t* nsab, int32_t* block_table, uint8_t* 
     allocate_blocks_kernel<<<1, 1024, smem, (cudaStream_t)stream>>>(nsab, block_table, is_free, seq_ids, target_lens, batch,
                                                                    block_size, num_blocks, mbps, new_out, cap, status);
     return check_launch("allocate_blocks_for_seqs");
+}
+
+int sllm_fork_blocks_for_seqs(int32_t* nsab, int32_t* block_table, int32_t* extra_refs, const int32_t* src_seq_ids,
+                              const int32_t* dst_seq_ids, const int32_t* lens, int batch, int block_size, int mbps,
+                              sllm_stream_t stream) {
+    SLLM_REQUIRE(batch >= 0 && block_size > 0 && mbps > 0, "fork_blocks: bad sizes");
+    if (batch == 0) return 0;
+    SLLM_REQUIRE(nsab && block_table && extra_refs && src_seq_ids && dst_seq_ids && lens, "fork_blocks: null pointer");
+    fork_blocks_kernel<<<cdiv(batch, 4), 128, 0, (cudaStream_t)stream>>>(nsab, block_table, extra_refs, src_seq_ids, dst_seq_ids,
+                                                                         lens, batch, block_size, mbps);
+    return check_launch("fork_blocks_for_seqs");
+}
+
+int sllm_copy_block_tails(void* k_cache, void* v_cache, int32_t* token_cache, const int32_t* block_table,
+                          const int32_t* src_seq_ids, const int32_t* dst_seq_ids, const int32_t* lens, int batch,
+                          int64_t block_bytes, int block_size, int mbps, sllm_stream_t stream) {
+    SLLM_REQUIRE(batch >= 0 && block_size > 0 && mbps > 0 && block_bytes > 0 && block_bytes % 16 == 0,
+                 "copy_block_tails: bad sizes (block_bytes %lld must be a positive multiple of 16)", (long long)block_bytes);
+    if (batch == 0) return 0;
+    SLLM_REQUIRE(k_cache && v_cache && block_table && src_seq_ids && dst_seq_ids && lens, "copy_block_tails: null pointer");
+    SLLM_REQUIRE(batch <= 65535, "copy_block_tails: batch %d too large", batch);
+    dim3 grid(cdiv(block_bytes, kTailChunk), batch, 2);
+    copy_block_tails_kernel<<<grid, kTailThreads, 0, (cudaStream_t)stream>>>(
+        (char*)k_cache, (char*)v_cache, token_cache, block_table, src_seq_ids, dst_seq_ids, lens, block_bytes, block_size, mbps);
+    return check_launch("copy_block_tails");
+}
+
+int sllm_release_blocks_for_seqs(int32_t* nsab, const int32_t* block_table, uint8_t* is_free, int32_t* extra_refs,
+                                 const int32_t* seq_ids, const int32_t* cumsum, int32_t* gathered, int batch, int mbps,
+                                 sllm_stream_t stream) {
+    SLLM_REQUIRE(batch >= 0 && mbps > 0, "release_blocks: bad sizes");
+    if (batch == 0) return 0;
+    SLLM_REQUIRE(nsab && block_table && is_free && extra_refs && seq_ids, "release_blocks: null pointer");
+    SLLM_REQUIRE(!gathered || cumsum, "release_blocks: gathering needs the cumsum");
+    if (gathered)
+        release_blocks_kernel<true><<<cdiv(batch, 4), 128, 0, (cudaStream_t)stream>>>(nsab, block_table, is_free, extra_refs,
+                                                                                       seq_ids, cumsum, gathered, batch, mbps);
+    else
+        release_blocks_kernel<false><<<cdiv(batch, 4), 128, 0, (cudaStream_t)stream>>>(nsab, block_table, is_free, extra_refs,
+                                                                                        seq_ids, nullptr, nullptr, batch, mbps);
+    return check_launch("release_blocks_for_seqs");
 }
 
 }  // extern "C"

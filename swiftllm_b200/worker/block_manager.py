@@ -5,12 +5,22 @@ allocation order (lowest free id first, batch order) - block ids are bit-exact w
 allocation is ONE kernel launch with no host<->device sync (the reference does assert(...).all(), .item() and
 torch.nonzero, block_manager.py:50,70,75).  The host keeps a mirror of `num_seq_allocated_blocks` so that
 exhaustion is detected on the host (RuntimeError, as in the reference) without reading the device.
+
+Shared blocks (addition, `fork_blocks_for_seqs`): a fork makes another sequence's row point at the leading blocks of a row, and
+`block_extra_refs` counts the owners of each block beyond the first.  Shared blocks are always a prefix of every row that holds
+them.  Until the first fork nothing changes: the same kernels free and gather.  Afterwards release drops one owner per block and
+a block becomes free when its last owner lets go; the host keeps the sharing in logical handles (per sequence, the handles of its
+leading blocks that have been shared; handle -> the sequences holding it), so `num_free_blocks` and the number of leading shared
+blocks of each sequence (`_host_shared`) stay exact without reading the device.  A call updates `_host_shared` only for the rows
+whose count it can change, so its host cost does not grow with the number of other live forks.
 """
 import numpy as np
 import torch
 
 from .kernels.block_mgmt import (allocate_blocks_for_seqs as _allocate_kernel,
+                                 fork_blocks_for_seqs as _fork_kernel,
                                  gather_allocated_blocks_and_unset,
+                                 release_blocks_for_seqs as _release_kernel,
                                  truncate_blocks_for_seqs as _truncate_kernel,
                                  unset_block_table_and_num_seq_alloc_blocks)
 
@@ -33,6 +43,14 @@ class BlockManager:
 
         self._host_nsab = np.zeros((max_seqs_in_block_table,), dtype=np.int64)   # host mirror
         self._status = torch.zeros((2,), dtype=torch.int32, device=device)
+
+        # block_id |-> owners beyond the first (0 for every free block)
+        self.block_extra_refs = torch.zeros((num_blocks,), dtype=torch.int32, device=device)
+        self.forked = False             # release is refcount-aware from the first fork on
+        self._rows = {}                 # seq_id |-> handles of its leading blocks that have been shared
+        self._holders = {}              # handle |-> set of the seq_ids holding it (its owners)
+        self._next_handle = 0
+        self._host_shared = np.zeros((max_seqs_in_block_table,), dtype=np.int64)   # leading blocks with > 1 owner
 
     @staticmethod
     def _to_list(t, given):
@@ -70,6 +88,63 @@ class BlockManager:
             self.num_free_blocks -= total
         return new_blocks
 
+    def fork_blocks_for_seqs(self, src_seq_ids: torch.Tensor, dst_seq_ids: torch.Tensor, lens: torch.Tensor, *,
+                             src_seq_ids_list, dst_seq_ids_list, lens_list):
+        """dst #i gets the first lens[i] // block_size blocks of src #i (shared, one more owner each) and, when lens[i] is not a
+        multiple of block_size, one fresh block allocated like any other (lowest free id first, batch order).  The caller has
+        validated the lists (empty, distinct dst rows that are no src; 1 <= lens[i] <= blocks held by src * block_size) and copies
+        the tail pages.  Raises RuntimeError, before any device work, when the tail blocks do not fit."""
+        bs = self.block_size
+        tails = sum(1 for p in lens_list if p % bs)
+        if tails > self.num_free_blocks:
+            raise RuntimeError(f"No enough free blocks available on {self.device_name} ({self.num_blocks} in total, "
+                               f"{self.num_free_blocks} free, {tails} requested)")
+        for s, d, p in zip(src_seq_ids_list, dst_seq_ids_list, lens_list):
+            k = p // bs
+            row = self._rows.setdefault(s, [])
+            while len(row) < k:             # blocks of src shared for the first time
+                self._holders[self._next_handle] = {s}
+                row.append(self._next_handle)
+                self._next_handle += 1
+            self._rows[d] = row[:k]
+            for h in row[:k]:
+                self._holders[h].add(d)
+            self._host_nsab[d] = k
+        self.forked = True
+        _fork_kernel(self.num_seq_allocated_blocks, self.block_table, self.block_extra_refs, src_seq_ids, dst_seq_ids, lens, bs)
+        self.allocate_blocks_for_seqs(dst_seq_ids, lens, seq_ids_list=dst_seq_ids_list, target_lens_list=lens_list,
+                                      want_new_blocks=False)
+        # a handle that gains an owner had one (src) or already counted as shared: only src and dst rows change
+        self._refresh_shared(set(src_seq_ids_list) | set(dst_seq_ids_list))
+
+    def _refresh_shared(self, sids):
+        """Recount the leading shared blocks of the given sequences."""
+        for sid in sids:
+            row = self._rows.get(sid, ())
+            n = 0
+            while n < len(row) and len(self._holders[row[n]]) > 1:
+                n += 1
+            self._host_shared[sid] = n
+
+    def _release_host(self, sids) -> int:
+        """Host side of a refcount-aware release: drop one owner of every block of the sequences; returns how many become free."""
+        freed, changed = 0, set()
+        for s in sids:
+            row = self._rows.pop(s, [])
+            freed += int(self._host_nsab[s]) - len(row)
+            for h in row:
+                holders = self._holders[h]
+                holders.discard(s)
+                if not holders:
+                    del self._holders[h]
+                    freed += 1
+                elif len(holders) == 1:     # its last holder no longer shares it
+                    changed |= holders
+            self._host_nsab[s] = 0
+            changed.add(s)
+        self._refresh_shared(changed)
+        return freed
+
     def truncate_blocks_for_seqs(self, seq_ids: torch.Tensor, target_lens: torch.Tensor, *, seq_ids_list=None,
                                  target_lens_list=None):
         """Shrink seq #i to ceil(target_lens[i] / block_size) blocks; the blocks past it become free (and are handed out again
@@ -86,6 +161,16 @@ class BlockManager:
         total = int((have - target).sum())
         if total == 0:
             return
+        if self.forked:
+            # every position a step writes lies past the sequence's shared blocks and a truncation keeps at least one written
+            # position, so only private blocks are given back: the plain truncation kernel stays correct
+            assert (target >= self._host_shared[idx]).all(), \
+                f"(On {self.device_name}) Logic error: truncating into blocks shared with a fork."
+            for s, t in zip(sids, target.tolist()):
+                for h in self._rows.get(s, [])[t:]:
+                    del self._holders[h]
+                if s in self._rows:
+                    del self._rows[s][t:]
         _truncate_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free,
                          seq_ids.to(torch.int32).contiguous(), target_lens.to(torch.int32).contiguous(), self.block_size)
         self._host_nsab[idx] = target
@@ -106,6 +191,11 @@ class BlockManager:
         total = int(self._host_nsab[idx].sum())
         if total == 0:
             return                      # nothing allocated for these sequences on this device
+        if self.forked:
+            self.num_free_blocks += self._release_host(sids)
+            _release_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free, self.block_extra_refs,
+                            seq_ids.to(torch.int32))
+            return
         self.num_free_blocks += total
         self._host_nsab[idx] = 0
         unset_block_table_and_num_seq_alloc_blocks(self.num_seq_allocated_blocks, self.block_table,
@@ -115,6 +205,10 @@ class BlockManager:
         sids = self._to_list(seq_ids, seq_ids_list)
         idx = np.asarray(sids, dtype=np.int64)
         total = int(self._host_nsab[idx].sum()) if sids else 0
+        if self.forked and sids:
+            self.num_free_blocks += self._release_host(sids)
+            return _release_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free, self.block_extra_refs,
+                                   seq_ids.to(torch.int32), total_blocks=total)
         gathered = gather_allocated_blocks_and_unset(self.num_seq_allocated_blocks, self.block_table,
                                                      seq_ids.to(torch.int32), self.is_block_free, total_blocks=total)
         if sids:

@@ -6,6 +6,7 @@
     forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities)
     forward_speculative(input_ids_list, seq_ids_list, prefix_lens_list, sampling_params_list=None) -> list[list[int]]
                                                             (addition: verify up to 7 drafts per sequence in one step)
+    fork_seqs(src_seq_ids_list, dst_seq_ids_list, lens_list)  (addition: share a cached prefix with another sequence)
     swap_in_seqs / swap_out_seqs / free_seqs_resources
 
 and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).  Addition: the token
@@ -33,6 +34,7 @@ from swiftllm_b200.model_config import LlamaModelConfig
 from swiftllm_b200.sampling_params import TokenLogprobs, has_penalties, logprobs_top_n, sampling_words
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
+from swiftllm_b200.worker.kernels.block_mgmt import copy_block_tails
 from swiftllm_b200.worker.weight import load_weights
 
 from .infer_state import LlamaInferState, SamplingState
@@ -396,6 +398,7 @@ class LlamaModel:
             raise ValueError("forward_speculative does not apply penalties (their history is per position)")
         if B == 0:
             return []
+        self._check_shared_writes(seq_ids_list, prefix)
         mc = self.model_config
         T = sum(rows)
         rep = np.repeat(np.arange(B), rows)
@@ -484,6 +487,8 @@ class LlamaModel:
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
                                               top_n, penalized, sampled)
 
+        if not ignore_kvcache:
+            self._check_shared_writes(seq_ids_list, prefix_lens + [l - 1 for l in decoding_seq_lens_list])
         # the sampling words go first: the int64 seeds need an 8-byte aligned offset
         views = self._stage_metadata(
             *([samp[0]] if samp else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens, prefill_starts, positions,
@@ -532,6 +537,7 @@ class LlamaModel:
         with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
         penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples)."""
         from swiftllm_b200 import _lib
+        self._check_shared_writes(seq_ids_list, [l - 1 for l in lens_list])
         B = len(flat_ids)
         mc = self.model_config
         nkv = mc.num_kv_heads // self.tp_size
@@ -649,6 +655,69 @@ class LlamaModel:
         tokens, logprobs = (out, None) if top_n is None else (out[0], out[1:])
         # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph
         return dict(graph=graph, meta=meta, host=host, next=0, tokens=tokens, logprobs=logprobs, keep=(last, empty))
+
+    # ------------------------------------------------------------------ shared blocks
+    def _check_shared_writes(self, seq_ids_list, first_positions):
+        """ValueError (before anything is enqueued) when a step would store K/V inside a block its sequence shares with a fork.
+        An entry writes the positions from first_positions[i] on, and shared blocks are the leading blocks of a row, so one
+        comparison per entry decides it.  Nothing to check until the first fork."""
+        bm = self.gpu_block_manager
+        if not bm.forked or len(seq_ids_list) == 0:
+            return
+        idx = np.asarray(seq_ids_list, dtype=np.int64)
+        pos = np.asarray(first_positions, dtype=np.int64)
+        bad = pos // bm.block_size < bm._host_shared[idx]
+        if bad.any():
+            i = int(np.argmax(bad))
+            raise ValueError(f"sequence {int(idx[i])} would write position {int(pos[i])}, inside one of its first "
+                             f"{int(bm._host_shared[idx[i]])} blocks, which it shares with a fork: shared blocks are read-only")
+
+    @torch.inference_mode()
+    def fork_seqs(self, src_seq_ids_list: list, dst_seq_ids_list: list, lens_list: list):
+        """Entry i: dst_seq_ids_list[i] holds the first P = lens_list[i] cached tokens of src_seq_ids_list[i], as if they had been
+        prefilled into it.  Blocks [0, P // block_size) of src are shared (dst's block-table row points at them, one more owner
+        each); when P % block_size != 0, dst gets a fresh block (lowest free id first, batch order) into which src's block
+        P // block_size is copied: K and V pages of every layer on this rank and the token page penalties read.  dst then continues
+        like any sequence: forward() decode at decoding_seq_len P + 1, chunked prefill with prefill_prefix_lens_list [P], or
+        forward_speculative at prefix P.  Several entries may fork the same src (n-way fork), and P may be shorter than what src
+        holds.  Sampling is a pure function of (logits, parameters, seed, position): forks decoded with the same fixed seed
+        produce identical continuations; parallel sampling uses seed=None or distinct seeds.
+
+        No step may store K/V inside a block that has more than one owner (ValueError before anything is enqueued); a block is
+        freed when its last owner is freed or swapped out, and a swapped-out fork comes back with private blocks.  Raises
+        ValueError, before anything is enqueued, when the list lengths differ, P < 1 or P > blocks held by src * block_size, src
+        holds no GPU blocks (or is swapped out), dst holds blocks on either device, a dst repeats or is also a src, or an id is
+        outside [0, max_seqs_in_block_table); RuntimeError when the tail blocks do not fit.  Stream-ordered, no host sync."""
+        B = len(src_seq_ids_list)
+        if len(dst_seq_ids_list) != B or len(lens_list) != B:
+            raise ValueError(f"fork_seqs: {B} sources but {len(dst_seq_ids_list)} destinations and {len(lens_list)} lengths")
+        src, dst, lens = ([int(x) for x in l] for l in (src_seq_ids_list, dst_seq_ids_list, lens_list))
+        gpu, cpu = self.gpu_block_manager, self.cpu_block_manager
+        bs, nseq = gpu.block_size, len(gpu._host_nsab)
+        for sid in src + dst:
+            if not 0 <= sid < nseq:
+                raise ValueError(f"fork_seqs: sequence id {sid} outside [0, {nseq})")
+        if len(set(dst)) != B:
+            raise ValueError("fork_seqs: a destination sequence repeats")
+        if set(dst) & set(src):
+            raise ValueError(f"fork_seqs: sequences {sorted(set(dst) & set(src))} are both a source and a destination")
+        for s, d, p in zip(src, dst, lens):
+            if cpu._host_nsab[s] > 0:
+                raise ValueError(f"fork_seqs: source sequence {s} is swapped out")
+            have = int(gpu._host_nsab[s])
+            if have == 0:
+                raise ValueError(f"fork_seqs: source sequence {s} holds no GPU blocks")
+            if not 1 <= p <= have * bs:
+                raise ValueError(f"fork_seqs: length {p} outside [1, {have * bs}] for source sequence {s} ({have} blocks)")
+            if gpu._host_nsab[d] > 0 or cpu._host_nsab[d] > 0:
+                raise ValueError(f"fork_seqs: destination sequence {d} already holds blocks")
+        if B == 0:
+            return
+        src_t, dst_t, lens_t = self._stage_metadata(src, dst, lens)
+        gpu.fork_blocks_for_seqs(src_t, dst_t, lens_t, src_seq_ids_list=src, dst_seq_ids_list=dst, lens_list=lens)
+        if any(p % bs for p in lens):
+            self._wait_for_swaps()      # pending swap copies may still read or write these pages
+            copy_block_tails(self.k_cache, self.v_cache, self.token_cache, gpu.block_table, src_t, dst_t, lens_t, bs)
 
     # ------------------------------------------------------------------ swap / free
     def _swap(self, seq_ids_list: list, is_swap_in: bool):
