@@ -411,7 +411,10 @@ int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* 
     SLLM_REQUIRE(block_size > 0 && num_layers > 0 && cur_layer >= 0 && cur_layer < num_layers && max_blocks_per_seq > 0 && num_blocks > 0,
                  "paged_attention_verify: bad cache geometry (layer %d of %d)", cur_layer, num_layers);
     cudaStream_t st = (cudaStream_t)stream;
-    if (dtype <= SLLM_BF16 && tc_verify_supported(head_dim, block_size, nq, nkv, max_rows, num_blocks, num_layers, num_tokens)) {
+    // SLLM_PAGED_ATTN_GEN=1 forces the paged-prefill kernel below, =2 makes a shape the verify kernel does not serve an error
+    const int gen = forced_generation();
+    if (gen != 1 && dtype <= SLLM_BF16 &&
+        tc_verify_supported(head_dim, block_size, nq, nkv, max_rows, num_blocks, num_layers, num_tokens)) {
         const int split_tokens = choose_split_tokens(num_seqs, nkv, max_seq_len, 0);
         const int num_splits = (max_seq_len + split_tokens - 1) / split_tokens;
         float *part_o = nullptr, *part_lse = nullptr;
@@ -437,6 +440,7 @@ int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* 
         }
         return 0;
     }
+    SLLM_REQUIRE(gen != 2, "paged_attention_verify: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma verify kernel");
     // shapes the verify kernel does not serve: the chunked-prefill kernel computes the same function (rows = chunk tokens)
     return sllm_prefill_attention_paged(q, k_cache, v_cache, o, block_table, seq_ids, start_locs, row_counts, prefix_lens,
                                         softmax_scale, num_seqs, max_rows, num_tokens, cur_layer, num_layers, nq, nkv, block_size,

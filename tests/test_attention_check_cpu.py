@@ -6,7 +6,10 @@ passes the check, and each fault model a kernel could plausibly commit fails it:
   * the last partial page (block_size 16 or 32) dropped;
   * an off-by-one causal mask, in both directions (prefill);
   * a wrong kv head: h // 8 or h // 16 (the padded group width of the wgmma decode kernel) instead of h // g;
-  * one head's output written over its neighbour's."""
+  * one head's output written over its neighbour's;
+and, for speculative verification (entries of 1-8 rows after a cached prefix, tests/test_speculative_gpu.py):
+  * every row of an entry sees the whole entry (masked by the entry's length instead of the row's position);
+  * row j's output written to row j + 1 of its entry (a wrong (row, head) column decode)."""
 import functools
 
 import numpy as np
@@ -15,6 +18,7 @@ import torch
 
 from attention_check import TOL, check_attention
 from oracle import kernels as K
+from verify_shapes import LAYOUTS, VERIFY_GEOMS, verify_layout
 
 DTYPES = [torch.float16, torch.bfloat16]
 LOG2E = 1.4426950408889634
@@ -29,8 +33,6 @@ PREFILL_GEOMS = [(4, 2, 64), (8, 2, 128), (4, 4, 128), (12, 4, 64), (24, 8, 128)
 PREFILL_LENS = [1, 2, 63, 64, 65, 127, 128, 129, 255, 256, 257, 300, 513, 700]
 PAGED_PREFIX = [0, 13, 64, 500, 100, 3, 255, 0]                          # test_prefill_attention_paged_vs_exact_oracle
 PAGED_CHUNK = [37, 200, 64, 1, 513, 2, 257, 300]
-
-
 def _padded_group(g):
     return 8 if g <= 8 else 16
 
@@ -149,13 +151,20 @@ def wrong_kv_head(c, L, pos):
     return dict(kv_of_head=torch.arange(c.nq) // _padded_group(c.nq // c.nkv))
 
 
+def whole_entry(c, L, pos):
+    """Every row sees all L keys of its entry: the causal mask taken from the entry's length, not the row's position."""
+    return dict(visible=torch.ones(len(pos), L, dtype=torch.bool))
+
+
 FAULTS = {"slip_one_split": slip_one_split, "drop_last_tile": drop_last_tile, "drop_last_partial_page": drop_last_partial_page,
           "causal_one_short": causal_one_short, "causal_one_long": causal_one_long, "wrong_kv_head": wrong_kv_head,
-          "head_to_neighbour": None}
+          "head_to_neighbour": None, "whole_entry": whole_entry, "row_to_next_row": None}
 APPLIES = {"decode": ["slip_one_split", "drop_last_tile", "drop_last_partial_page", "wrong_kv_head", "head_to_neighbour"],
            "prefill": ["slip_one_split", "drop_last_tile", "causal_one_short", "causal_one_long", "wrong_kv_head",
                        "head_to_neighbour"],
-           "paged_prefill": list(FAULTS)}
+           "paged_prefill": ["slip_one_split", "drop_last_tile", "drop_last_partial_page", "causal_one_short", "causal_one_long",
+                             "wrong_kv_head", "head_to_neighbour"],
+           "verify": list(FAULTS)}
 
 
 def _faulty(case, name):
@@ -164,13 +173,19 @@ def _faulty(case, name):
         h = case.nq // 2 - 1
         o[:, h + 1] = o[:, h]
         return o
+    if name == "row_to_next_row":          # row j of each entry lands on row j + 1 (row 0 keeps its own output)
+        o = case.run(case.dtype).clone()
+        for s0, n in zip(case.starts, case.lens):
+            o[s0 + 1:s0 + n] = o[s0:s0 + n - 1].clone()
+        return o
     return case.run(case.dtype, FAULTS[name])
 
 
 # ----------------------------------------------------------------------------- shapes
 SHAPES = ([("decode", g, None) for g in DECODE_GEOMS] + [("decode", (32, 8, 128), "full")] +
           [("prefill", g, None) for g in PREFILL_GEOMS] +
-          [("paged_prefill", g, 16) for g in PREFILL_GEOMS] + [("paged_prefill", (8, 2, 128), 32)])
+          [("paged_prefill", g, 16) for g in PREFILL_GEOMS] + [("paged_prefill", (8, 2, 128), 32)] +
+          [("verify", (g * nkv, nkv, 128), (r, lay)) for g, nkv, r, _ in VERIFY_GEOMS for lay in LAYOUTS])
 
 
 @functools.lru_cache(maxsize=None)
@@ -181,11 +196,16 @@ def _case(kind, geom, extra, dtype):
         return Case(kind, nq, nkv, D, dtype, FULL_LENS if extra == "full" else DECODE_LENS, seed=seed)
     if kind == "prefill":
         return Case(kind, nq, nkv, D, dtype, PREFILL_LENS, seed=seed)
+    if kind == "verify":
+        rows, prefix = verify_layout(extra[1], nq // nkv, extra[0])
+        return Case(kind, nq, nkv, D, dtype, rows, prefix=prefix, seed=seed + extra[0])
     return Case(kind, nq, nkv, D, dtype, PAGED_CHUNK, prefix=PAGED_PREFIX, bs=extra, seed=seed)
 
 
 def _id(s):
     kind, (nq, nkv, D), extra = s
+    if kind == "verify":
+        extra = f"{extra[0]}rows-{extra[1]}"
     return f"{kind}-{nq}q{nkv}kv-d{D}" + (f"-{extra}" if extra is not None else "")
 
 
@@ -199,7 +219,9 @@ def test_kernel_rounding_passes(shape, dtype, m_ref):
 
 
 def _applies(shape, fault):
-    kind, (nq, nkv, D), _ = shape
+    kind, (nq, nkv, D), extra = shape
+    if kind == "verify" and extra[0] == 1 and fault in ("causal_one_long", "whole_entry", "row_to_next_row"):
+        return False                      # 1-row entries: the row is the last position, there is no later row or key
     if fault == "wrong_kv_head":          # only where h // NP differs from h // g for some head
         return not torch.equal(torch.arange(nq) // _padded_group(nq // nkv), torch.arange(nq) // (nq // nkv))
     return fault in APPLIES[kind]

@@ -1,5 +1,6 @@
 """GPU: speculative verification - the multi-query paged-attention kernel (sllm_paged_attention_verify) against the fp64
 definition for every (entry, q head, row), and LlamaModel.forward_speculative end to end."""
+import functools
 from types import SimpleNamespace
 
 import numpy as np
@@ -11,6 +12,7 @@ from attention_check import TOL, check_attention
 from oracle import kernels as K
 from oracle.model import OracleLlama, OracleWeights
 from test_model_gpu import ENG2, TINY2, _make_model
+from verify_shapes import LAYOUTS, VERIFY_GEOMS, geom_id, random_kv_q, verify_layout, verify_np
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -21,9 +23,40 @@ def _i32(x):
     return torch.tensor(list(x), dtype=torch.int32, device=DEV)
 
 
+@pytest.fixture(params=["wgmma", "fallback"])
+def verify_gen(request, monkeypatch):
+    """Which kernel serves sllm_paged_attention_verify: the wgmma verify kernel (SLLM_PAGED_ATTN_GEN=2, where a shape it does
+    not serve is an error) or the paged-prefill kernel it falls back to (=1).  The 1-row decode comparisons then run the
+    wgmma decode kernel and the mma.sync decode kernel respectively."""
+    monkeypatch.setenv("SLLM_PAGED_ATTN_GEN", "2" if request.param == "wgmma" else "1")
+    return request.param
+
+
+def fused_q(q, nkv):
+    """q [T, nq, D] as the column slice of a [T, (nq + 2 nkv) D] buffer (the fused QKV GEMM's output) whose k / v columns
+    hold NaN: the kernel sees q's row stride (nq + 2 nkv) D and must never read past q's own columns."""
+    T, nq, D_ = q.shape
+    buf = torch.full((T, (nq + 2 * nkv) * D_), float("nan"), dtype=q.dtype, device=q.device)
+    buf[:, :nq * D_] = q.reshape(T, -1)
+    return buf[:, :nq * D_].unflatten(1, (nq, D_))
+
+
 def _case(g_, nkv, rows, prefix, dtype, seed, mbps=None):
     """Random caches (2 layers, layer 1 used), a block table over randomly permuted block ids with entry i in table row 2 i + 1,
-    packed q; returns the device tensors, the metadata and the fp64 output."""
+    packed q; returns the device tensors, the metadata and the fp64 output.  rows / prefix: tuples."""
+    c = _inputs(g_, nkv, rows, prefix, dtype, seed, mbps)
+    o64 = _exact(g_, nkv, rows, prefix, dtype, seed, mbps)
+    return dict(c, q=c["q"].to(DEV), kc=c["kc"].to(DEV), vc=c["vc"].to(DEV), bt=c["bt"].to(DEV), o64=o64)
+
+
+@functools.lru_cache(maxsize=None)        # the fp64 outputs (small) are shared by the two kernels
+def _exact(*key):
+    c = _inputs(*key)
+    return K.prefix_prefill_attention_exact(c["q"], c["kc"], c["vc"], c["bt"].numpy(), c["sids"], c["starts"], c["rows"],
+                                            c["prefix"], D ** -0.5, BS, LAYER)
+
+
+def _inputs(g_, nkv, rows, prefix, dtype, seed, mbps):
     gen = torch.Generator().manual_seed(seed)
     nq = nkv * g_
     need = [(p + n + BS - 1) // BS for p, n in zip(prefix, rows)]
@@ -34,40 +67,38 @@ def _case(g_, nkv, rows, prefix, dtype, seed, mbps=None):
     at = 0
     for i, n in enumerate(need):
         bt[2 * i + 1, :n] = perm[at:at + n].to(torch.int32); at += n
-    kc = torch.randn(nblk, LAYERS, nkv, BS, D, generator=gen).to(dtype)
-    vc = torch.randn(nblk, LAYERS, nkv, BS, D, generator=gen).to(dtype)
-    T = sum(rows)
-    q = torch.randn(T, nq, D, generator=gen).to(dtype)
+    kc, vc, q = random_kv_q(gen, nblk, LAYERS, nkv, sum(rows), nq, D, BS, dtype)
     starts = list(np.cumsum([0] + list(rows[:-1])))
     sids = [2 * i + 1 for i in range(len(rows))]
-    o64 = K.prefix_prefill_attention_exact(q, kc, vc, bt.numpy(), sids, starts, rows, prefix, D ** -0.5, BS, LAYER)
-    return dict(q=q.to(DEV), kc=kc.to(DEV), vc=vc.to(DEV), bt=bt.to(DEV), sids=sids, starts=starts, rows=list(rows),
-                prefix=list(prefix), nq=nq, o64=o64)
+    return dict(q=q, kc=kc, vc=vc, bt=bt, sids=sids, starts=starts, rows=list(rows), prefix=list(prefix), nq=nq)
 
 
-def _verify(c):
+def _verify(c, q=None):
+    """paged_attention_verify on the case (q defaults to the case's contiguous q) into a NaN-filled output."""
     from swiftllm_b200.worker.kernels.prefill_attn import paged_attention_verify
+    q = c["q"] if q is None else q
     st = SimpleNamespace(seq_ids=_i32(c["sids"]), prefill_prefix_lens=_i32(c["prefix"]), num_prefill_seqs=len(c["rows"]),
                          max_prefill_kv_len=max(p + n for p, n in zip(c["prefix"], c["rows"])),
                          prefill_seq_start_locs=_i32(c["starts"]), prefill_seq_lens=_i32(c["rows"]), max_prefill_len=max(c["rows"]),
                          softmax_scale=D ** -0.5)
-    o = torch.full_like(c["q"], float("nan"))
-    paged_attention_verify(c["q"], c["kc"], c["vc"], c["bt"], o, None, None, st, LAYER)
+    o = torch.full(q.shape, float("nan"), dtype=q.dtype, device=DEV)
+    paged_attention_verify(q, c["kc"], c["vc"], c["bt"], o, None, None, st, LAYER)
     torch.cuda.synchronize()
     return o
 
 
-def _paged(c, idx):
-    """sllm_paged_attention on the given 1-row entries (decode at position prefix)."""
+def _paged_rows(c):
+    """sllm_paged_attention with every row as a decode sequence: row j of entry i at length prefix_i + j + 1."""
     from swiftllm_b200.worker.kernels.paged_attn import paged_attention
-    lens = [c["prefix"][i] + 1 for i in idx]
-    st = SimpleNamespace(paged_attn_seq_block_size=0, seq_ids=_i32([c["sids"][i] for i in idx]), num_prefill_seqs=0,
+    sids = [s for s, n in zip(c["sids"], c["rows"]) for _ in range(n)]
+    lens = [p + j + 1 for p, n in zip(c["prefix"], c["rows"]) for j in range(n)]
+    st = SimpleNamespace(paged_attn_seq_block_size=0, seq_ids=_i32(sids), num_prefill_seqs=0,
                          decoding_seq_lens=_i32(lens), max_decoding_len=max(lens), softmax_scale=D ** -0.5)
-    q = c["q"][[c["starts"][i] for i in idx]].contiguous()
-    o = torch.empty((len(idx), c["nq"] * D), dtype=q.dtype, device=DEV)
+    q = c["q"].contiguous()
+    o = torch.empty((q.shape[0], c["nq"] * D), dtype=q.dtype, device=DEV)
     paged_attention(q, c["kc"], c["vc"], c["bt"], None, SimpleNamespace(block_size=BS), st, LAYER, o)
     torch.cuda.synchronize()
-    return o
+    return o, lens
 
 
 def _workspace_splits(c, nkv):
@@ -78,66 +109,66 @@ def _workspace_splits(c, nkv):
     return 1 if ws == 0 else (ws - 4 * T) // (T * c["nq"] * (D + 1) * 4)
 
 
-def _short_many(rng):
-    """48 entries, ragged rows 1..8, prefixes at page edges and small random ones: one split per item."""
-    rows = [1 + i % 8 for i in range(48)]
-    prefix = rng.integers(0, 300, size=48).tolist()
-    prefix[:6] = [0, 1, 15, 16, 17, 31]
-    return rows, prefix
-
-
-def _long_few(rng):
-    """Three long entries (several splits): columns of early rows see nothing of the last split; the second entry ends exactly
-    at the last slot of its max_blocks_per_seq table row."""
-    return [8, 5, 1], [3001, 4096 - 5, 17]
-
-
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["fp16", "bf16"])
-@pytest.mark.parametrize("g_,max_rows", [(1, 8), (4, 8), (8, 4), (8, 8)], ids=["g1", "g4", "g8-4rows", "g8-fallback"])
-@pytest.mark.parametrize("regime", ["short_many", "long_few"])
-def test_verify_kernel_vs_fp64(dtype, g_, max_rows, regime):
-    """Every (entry, q head, row) within the decode-attention tolerance of fp64; g * rows <= 32 runs the multi-query kernel,
-    g8 with 8 rows the chunked-prefill kernel.  Rows of 1-row entries also agree with sllm_paged_attention."""
-    rng = np.random.default_rng(10 * g_ + max_rows)
-    rows, prefix = (_short_many if regime == "short_many" else _long_few)(rng)
-    rows = [min(r, max_rows) for r in rows]
-    nkv = 8
+@pytest.mark.parametrize("geom", VERIFY_GEOMS, ids=geom_id)
+@pytest.mark.parametrize("regime", LAYOUTS)
+def test_verify_kernel_vs_fp64(dtype, geom, regime, verify_gen):
+    """Every (entry, q head, row) within the decode-attention tolerance of fp64, under both kernels; under `wgmma` a shape of
+    more than 32 columns must be refused.  q is a column slice of a fused QKV buffer (NaN k / v columns) in short_many and
+    contiguous in long_few.  Row j of every entry also agrees with sllm_paged_attention at length prefix + j + 1."""
+    g_, nkv, max_rows, npad = geom
+    rows, prefix = verify_layout(regime, g_, max_rows)
+    rows = tuple(rows)
+    assert verify_np(g_, max(rows)) == npad, "the rows must give the launch the intended wgmma width"
     mbps = 256 if regime == "long_few" else None
-    c = _case(g_, nkv, rows, prefix, dtype, seed=3, mbps=mbps)
+    c = _case(g_, nkv, rows, tuple(prefix), dtype, seed=3, mbps=mbps)
     if regime == "long_few":
         assert _workspace_splits(c, nkv) > 1
-    o = _verify(c)
-    check_attention(o, c["o64"], c["nq"], c["rows"], starts=c["starts"], prefix=c["prefix"], what="paged_attention_verify")
-    one = [i for i, n in enumerate(rows) if n == 1]
-    if one:
-        op = _paged(c, one)
-        ov = o[[c["starts"][i] for i in one]].reshape(len(one), -1)
-        check_attention(ov, op.double(), c["nq"], tol=2 * TOL[dtype], what="verify vs paged_attention")
+    q = fused_q(c["q"], nkv) if regime == "short_many" else c["q"]
+    if verify_gen == "wgmma" and npad is None:
+        with pytest.raises(RuntimeError, match="SLLM_PAGED_ATTN_GEN=2"):
+            _verify(c, q)
+        return
+    o = _verify(c, q)
+    check_attention(o, c["o64"], c["nq"], c["rows"], starts=c["starts"], prefix=c["prefix"],
+                    what=f"paged_attention_verify(wgmma, np{npad})" if verify_gen == "wgmma" else "paged_attention_verify(fallback)")
+    op, lens = _paged_rows(c)
+    check_attention(o.reshape(len(lens), -1), op.double(), c["nq"], lens, tol=2 * TOL[dtype], what="verify vs paged_attention")
 
 
-def _oracle(w, tdt):
-    return OracleLlama(TINY2, w, block_size=16, num_blocks=ENG2["num_blocks"], num_cpu_blocks=4, max_seqs_in_block_table=16,
+def _oracle(w, tdt, cfg=TINY2):
+    return OracleLlama(cfg, w, block_size=16, num_blocks=ENG2["num_blocks"], num_cpu_blocks=4, max_seqs_in_block_table=16,
                        max_blocks_per_seq=16, attn="exact", dtype=tdt)
+
+
+# GQA group 3 at head_dim 128 (12 q / 4 kv heads): the verify kernel runs with 8 dead columns at 8 rows (N = 32) and one at
+# 5 rows (N = 16), on q sliced from the fused QKV output
+TINY3 = dict(TINY2, num_attention_heads=12, num_key_value_heads=4, hidden_size=1536)
+E2E_CASES = {"g4-np32": (TINY2, [8, 1, 5], 32), "g3-np32": (TINY3, [8, 1, 5], 32), "g3-np16": (TINY3, [5, 1, 3], 16)}
 
 
 @pytest.mark.parametrize("dtype", ["bfloat16", "float16"])
 @pytest.mark.parametrize("sampled", [False, True], ids=["greedy", "sampled"])
-def test_forward_speculative_end_to_end(dtype, sampled):
+@pytest.mark.parametrize("model", list(E2E_CASES))
+def test_forward_speculative_end_to_end(dtype, sampled, model, monkeypatch):
     """Per-row logits within test_model_gpu's tolerance of the oracle fed the rows one at a time; greedy tokens equal the
     oracle's where the top-1 margin is clear; sampled tokens equal the sampling restatement applied to the product's own logits
-    rows with pos = prefix + j + 1 (exact); the device block state matches the host mirror and ceil(len / bs) afterwards."""
+    rows with pos = prefix + j + 1 (exact); the device block state matches the host mirror and ceil(len / bs) afterwards.
+    The verify attention must be served by the wgmma verify kernel at the intended width."""
     from swiftllm_b200 import SamplingParams
+    cfg, rows, npad = E2E_CASES[model]
+    assert verify_np(cfg["num_attention_heads"] // cfg["num_key_value_heads"], max(rows)) == npad
+    monkeypatch.setenv("SLLM_PAGED_ATTN_GEN", "2")           # a shape the wgmma kernels do not serve is an error
     tdt = dict(bfloat16=torch.bfloat16, float16=torch.float16)[dtype]
     tol = 2 ** -5 if dtype == "bfloat16" else 4e-3
-    w = OracleWeights.random(TINY2, dtype=tdt, seed=3, std=0.05)
-    m, o = _make_model(TINY2, ENG2, w, dtype=dtype), _oracle(w, tdt)
+    w = OracleWeights.random(cfg, dtype=tdt, seed=3, std=0.05)
+    m, o = _make_model(cfg, ENG2, w, dtype=dtype), _oracle(w, tdt, cfg)
     rng = np.random.default_rng(2)
     plens = [15, 16, 33]
     sids = [7, 1, 4]
     prompts = [rng.integers(0, 1000, size=n).tolist() for n in plens]
     first = o.forward(prompts, sids, [])
     m.forward(prompts, sids, [])
-    rows = [8, 1, 5]
     entries = [[x] + rng.integers(0, 1000, size=n - 1).tolist() for x, n in zip(first, rows)]
     params = [SamplingParams(0.8, top_k=(0, 50, 0)[i], seed=9 + i) for i in range(3)] if sampled else None
     out = m.forward_speculative(entries, sids, plens, params)
