@@ -14,6 +14,7 @@
 #include <stdlib.h>
 
 #include "mma_helpers.cuh"
+#include "paged_attn_tc.cuh"      // generation 2
 
 namespace sllm {
 
@@ -246,6 +247,20 @@ __global__ void paged_attn_merge_kernel(const float* __restrict__ part_o, const 
     o[((int64_t)seq * nq + head) * D + d] = Traits<T>::from_f(O / L);
 }
 
+// `lens`: the visible length of each of the `rows` rows of o
+template <typename T>
+static int launch_merge(const float* part_o, const float* part_lse, void* o, const int32_t* lens, int nq, int64_t rows, int head_dim,
+                        int num_splits, int split_tokens, cudaStream_t stream, const char* what) {
+    dim3 grid(nq, (unsigned)rows);
+    paged_attn_merge_kernel<T><<<grid, head_dim, 0, stream>>>(part_o, part_lse, (T*)o, lens, nq, head_dim, num_splits, split_tokens);
+    return check_launch(what);
+}
+
+// bytes of the fp32 partials (normalised o + log2-sum-exp) of `rows` rows of o split `num_splits` ways
+static int64_t partial_bytes(int64_t rows, int nq, int64_t num_splits, int head_dim) {
+    return rows * nq * num_splits * (head_dim + 1) * (int64_t)sizeof(float);
+}
+
 // ---- host-side split policy (v1 vs v2)
 static int num_sms() {                       // of the CURRENT device (a process may drive several)
     static int sms[64] = {0};
@@ -272,21 +287,6 @@ static int choose_split_tokens(int num_seqs, int nkv, int max_seq_len, int seq_b
     return (int)st;
 }
 
-// generation 2 (paged_attn_tc.cu)
-bool tc_paged_supported(int head_dim, int block_size, int nq, int nkv, int64_t num_blocks, int num_layers);
-int launch_paged_tc(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table, const int32_t* seq_ids,
-                    const int32_t* seq_lens, void* o, float* part_o, float* part_lse, float scale_log2e, int num_seqs,
-                    int split_tokens, int num_splits, int cur_layer, int num_layers, int nq, int nkv, int max_blocks_per_seq,
-                    int64_t num_blocks, int64_t q_row_stride, sllm_dtype_t dtype, int num_sms, cudaStream_t stream);
-bool tc_verify_supported(int head_dim, int block_size, int nq, int nkv, int max_rows, int64_t num_blocks, int num_layers,
-                         int64_t num_tokens);
-int launch_paged_verify_tc(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table,
-                           const int32_t* seq_ids, const int32_t* start_locs, const int32_t* row_counts,
-                           const int32_t* prefix_lens, void* o, float* part_o, float* part_lse, int32_t* row_lens,
-                           float scale_log2e, int num_seqs, int max_rows, int64_t num_tokens, int split_tokens, int num_splits,
-                           int cur_layer, int num_layers, int nq, int nkv, int max_blocks_per_seq, int64_t num_blocks,
-                           int64_t q_row_stride, sllm_dtype_t dtype, int num_sms, cudaStream_t stream);
-
 // SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements, debugging); default: TMA/wgmma
 // whenever the shape is covered (head_dim 128, block_size 16).
 static int forced_generation() {
@@ -305,12 +305,9 @@ static int launch_paged(const PagedAttnParams& p, int num_seqs, int max_seq_len,
     paged_attn_kernel<T, D><<<grid, PA_THREADS, smem, stream>>>(p);
     int e = check_launch("paged_attention(phase 1)");
     if (e) return e;
-    if (p.num_splits > 1) {
-        dim3 g2(p.nq, num_seqs);
-        paged_attn_merge_kernel<T><<<g2, D, 0, stream>>>(p.part_o, p.part_lse, (T*)p.o, p.seq_lens, p.nq, D, p.num_splits,
-                                                         p.split_tokens);
-        return check_launch("paged_attention(phase 2)");
-    }
+    if (p.num_splits > 1)
+        return launch_merge<T>(p.part_o, p.part_lse, p.o, p.seq_lens, p.nq, num_seqs, D, p.num_splits, p.split_tokens, stream,
+                               "paged_attention(phase 2)");
     return 0;
 }
 
@@ -326,7 +323,7 @@ int64_t sllm_paged_attention_workspace_bytes(int num_decoding_seqs, int nq, int 
     const int st = choose_split_tokens(num_decoding_seqs, nkv, max_seq_len, seq_block_size);
     const int64_t ns = (max_seq_len + st - 1) / st;
     if (ns <= 1) return 0;
-    return (int64_t)num_decoding_seqs * nq * ns * (head_dim + 1) * (int64_t)sizeof(float);
+    return partial_bytes(num_decoding_seqs, nq, ns, head_dim);
 }
 
 int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_table,
@@ -355,7 +352,7 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
     p.max_blocks_per_seq = max_blocks_per_seq; p.q_stride = q_row_stride;
     p.part_o = nullptr; p.part_lse = nullptr;
     if (p.num_splits > 1) {
-        const int64_t need = (int64_t)num_decoding_seqs * nq * p.num_splits * (head_dim + 1) * (int64_t)sizeof(float);
+        const int64_t need = partial_bytes(num_decoding_seqs, nq, p.num_splits, head_dim);
         SLLM_REQUIRE(workspace && workspace_bytes >= need, "paged_attention: workspace too small (%lld < %lld bytes)",
                      (long long)workspace_bytes, (long long)need);
         p.part_o = (float*)workspace;
@@ -364,16 +361,18 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
     cudaStream_t st = (cudaStream_t)stream;
     if (forced_generation() != 1 && tc_paged_supported(head_dim, block_size, nq, nkv, num_blocks, num_layers) &&
         dtype <= SLLM_BF16) {
-        int e = launch_paged_tc(q, k_cache, v_cache, block_table, seq_ids, seq_lens, o, p.part_o, p.part_lse, p.scale_log2e,
-                                num_decoding_seqs, p.split_tokens, p.num_splits, cur_layer, num_layers, nq, nkv,
-                                max_blocks_per_seq, num_blocks, q_row_stride, dtype, num_sms(), st);
+        TcLaunch a = {};
+        a.p.block_table = block_table; a.p.seq_ids = seq_ids; a.p.seq_lens = seq_lens;
+        a.p.o = o; a.p.part_o = p.part_o; a.p.part_lse = p.part_lse; a.p.scale_log2e = p.scale_log2e;
+        a.p.split_tokens = p.split_tokens; a.p.num_splits = p.num_splits; a.p.cur_layer = cur_layer; a.p.num_layers = num_layers;
+        a.p.nq = nq; a.p.nkv = nkv; a.p.max_blocks_per_seq = max_blocks_per_seq;
+        a.q = q; a.k_cache = k_cache; a.v_cache = v_cache; a.num_blocks = num_blocks; a.q_row_stride = q_row_stride;
+        a.num_tokens = num_decoding_seqs; a.num_seqs = num_decoding_seqs; a.dtype = dtype; a.num_sms = num_sms(); a.stream = st;
+        int e = launch_paged_tc(a);
         if (e) return e;
-        if (p.num_splits > 1) {
-            dim3 g2(nq, num_decoding_seqs);
-            SLLM_DISPATCH_DTYPE(dtype, (paged_attn_merge_kernel<T><<<g2, head_dim, 0, st>>>(p.part_o, p.part_lse, (T*)o, seq_lens, nq,
-                                                                                          head_dim, p.num_splits, p.split_tokens)));
-            return check_launch("paged_attention(phase 2)");
-        }
+        if (p.num_splits > 1)
+            SLLM_DISPATCH_DTYPE(dtype, return (launch_merge<T>(p.part_o, p.part_lse, o, seq_lens, nq, num_decoding_seqs, head_dim,
+                                                               p.num_splits, p.split_tokens, st, "paged_attention(phase 2)")));
         return 0;
     }
     SLLM_REQUIRE(forced_generation() != 2, "paged_attention: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
@@ -390,7 +389,7 @@ int64_t sllm_paged_attention_verify_workspace_bytes(int num_seqs, int64_t num_to
     const int st = choose_split_tokens(num_seqs, nkv, max_seq_len, 0);
     const int64_t ns = (max_seq_len + st - 1) / st;
     if (ns <= 1) return 0;
-    return num_tokens * nq * ns * (head_dim + 1) * (int64_t)sizeof(float) + num_tokens * (int64_t)sizeof(int32_t);
+    return partial_bytes(num_tokens, nq, ns, head_dim) + num_tokens * (int64_t)sizeof(int32_t);
 }
 
 int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* v_cache, void* o, const int32_t* block_table,
@@ -427,17 +426,19 @@ int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* 
             part_lse = part_o + num_tokens * nq * num_splits * head_dim;
             row_lens = (int32_t*)(part_lse + num_tokens * nq * num_splits);
         }
-        int e = launch_paged_verify_tc(q, k_cache, v_cache, block_table, seq_ids, start_locs, row_counts, prefix_lens, o, part_o,
-                                       part_lse, row_lens, softmax_scale * 1.4426950408889634f, num_seqs, max_rows, num_tokens,
-                                       split_tokens, num_splits, cur_layer, num_layers, nq, nkv, max_blocks_per_seq, num_blocks,
-                                       q_row_stride, dtype, num_sms(), st);
+        TcLaunch a = {};
+        a.p.block_table = block_table; a.p.seq_ids = seq_ids; a.p.start_locs = start_locs; a.p.row_counts = row_counts;
+        a.p.prefix_lens = prefix_lens; a.p.o = o; a.p.part_o = part_o; a.p.part_lse = part_lse; a.p.row_lens = row_lens;
+        a.p.scale_log2e = softmax_scale * 1.4426950408889634f; a.p.split_tokens = split_tokens; a.p.num_splits = num_splits;
+        a.p.cur_layer = cur_layer; a.p.num_layers = num_layers; a.p.nq = nq; a.p.nkv = nkv;
+        a.p.max_blocks_per_seq = max_blocks_per_seq; a.p.qrows = max_rows;
+        a.q = q; a.k_cache = k_cache; a.v_cache = v_cache; a.num_blocks = num_blocks; a.q_row_stride = q_row_stride;
+        a.num_tokens = num_tokens; a.num_seqs = num_seqs; a.dtype = dtype; a.num_sms = num_sms(); a.stream = st;
+        int e = launch_paged_verify_tc(a);
         if (e) return e;
-        if (num_splits > 1) {
-            dim3 g2(nq, (unsigned)num_tokens);
-            SLLM_DISPATCH_DTYPE(dtype, (paged_attn_merge_kernel<T><<<g2, head_dim, 0, st>>>(part_o, part_lse, (T*)o, row_lens, nq,
-                                                                                          head_dim, num_splits, split_tokens)));
-            return check_launch("paged_attention_verify(merge)");
-        }
+        if (num_splits > 1)
+            SLLM_DISPATCH_DTYPE(dtype, return (launch_merge<T>(part_o, part_lse, o, row_lens, nq, num_tokens, head_dim, num_splits,
+                                                               split_tokens, st, "paged_attention_verify(merge)")));
         return 0;
     }
     SLLM_REQUIRE(gen != 2, "paged_attention_verify: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma verify kernel");

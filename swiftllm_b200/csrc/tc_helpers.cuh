@@ -179,7 +179,7 @@ __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
 typedef CUresult (*TensorMapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-TensorMapEncodeFn get_tensor_map_encoder();     // nullptr if unavailable (tc_host.cu)
+TensorMapEncodeFn get_tensor_map_encoder();     // nullptr if unavailable (host.cu)
 
 }  // namespace tc
 }  // namespace sllm
