@@ -15,6 +15,10 @@ namespace sllm {
 // ---------------------------------------------------------------- errors
 void set_error(const char* fmt, ...);
 int check_launch(const char* what);   // cudaGetLastError -> error code + message
+// Kernel generation forced by the environment variable `env_var`: "1" forces generation 1 (A/B measurements, debugging), "2"
+// makes a shape generation 2 does not serve an error, anything else 0 (generation 2 wherever it serves the shape).  Re-read on
+// every call, so tests can toggle it.
+int forced_generation(const char* env_var);
 
 #define SLLM_REQUIRE(cond, ...)            \
     do {                                   \

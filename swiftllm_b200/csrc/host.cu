@@ -1,6 +1,10 @@
-// Library plumbing (errors, device check) and the host-side block swapper.
+// Library plumbing (errors, device check, kernel-generation switch, tensor maps) and the host-side block swapper.
 #include <stdarg.h>
+#include <stdlib.h>
 
+#include <mutex>
+#include <string_view>
+#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
@@ -26,6 +30,11 @@ int check_launch(const char* what) {
     return 0;
 }
 
+int forced_generation(const char* env_var) {
+    const char* e = getenv(env_var);
+    return (e && e[0] == '1') ? 1 : (e && e[0] == '2') ? 2 : 0;
+}
+
 namespace tc {
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 TensorMapEncodeFn get_tensor_map_encoder() {
@@ -41,6 +50,49 @@ TensorMapEncodeFn get_tensor_map_encoder() {
         cudaGetLastError();
     }
     return fn;
+}
+
+bool encode_tma_map(CUtensorMap* out, const void* ptr, sllm_dtype_t dt, int rank, const cuuint64_t* dims,
+                    const cuuint64_t* byte_strides, const cuuint32_t* box) {
+    TensorMapEncodeFn enc = get_tensor_map_encoder();
+    if (!enc) return false;
+    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+    return enc(out, dt == SLLM_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr),
+               dims, byte_strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+namespace {
+struct MapKey {         // every argument of cached_tma_map, unused dimensions zero; compared and hashed as bytes
+    const void* ptr; int dt, rank; cuuint64_t dims[5], strides[4]; cuuint32_t box[5], unused;
+    std::string_view bytes() const { return std::string_view(reinterpret_cast<const char*>(this), sizeof(*this)); }
+    bool operator==(const MapKey& o) const { return bytes() == o.bytes(); }
+};
+static_assert(std::has_unique_object_representations_v<MapKey>, "MapKey must have no padding bytes");
+struct MapKeyHash { size_t operator()(const MapKey& k) const { return std::hash<std::string_view>()(k.bytes()); } };
+std::mutex g_map_mutex;
+std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
+}  // namespace
+
+bool cached_tma_map(CUtensorMap* out, const void* ptr, sllm_dtype_t dt, int rank, const cuuint64_t* dims,
+                    const cuuint64_t* byte_strides, const cuuint32_t* box) {
+    if (rank < 1 || rank > 5) return false;
+    MapKey key{};
+    key.ptr = ptr; key.dt = (int)dt; key.rank = rank;
+    for (int i = 0; i < rank; i++) {
+        key.dims[i] = dims[i]; key.box[i] = box[i];
+        if (i > 0) key.strides[i - 1] = byte_strides[i - 1];
+    }
+    {
+        std::lock_guard<std::mutex> lk(g_map_mutex);
+        auto it = g_maps.find(key);
+        if (it != g_maps.end()) { *out = it->second; return true; }
+    }
+    if (!encode_tma_map(out, ptr, dt, rank, dims, byte_strides, box)) return false;
+    std::lock_guard<std::mutex> lk(g_map_mutex);
+    if (g_maps.size() > 4096) g_maps.clear();
+    g_maps[key] = *out;
+    return true;
 }
 }  // namespace tc
 

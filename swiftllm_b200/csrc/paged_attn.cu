@@ -11,8 +11,6 @@
 //     merge kernel, same (normalised o, log2-sum-exp) partial format as the reference) otherwise.
 // HBM roofline: algorithmic bytes per launch = sum_i len_i * nkv * D * 2 (K and V) * sizeof(T)
 //               + 2 * Bd * nq * D * sizeof(T)  (SURVEY.md §8d).
-#include <stdlib.h>
-
 #include "mma_helpers.cuh"
 #include "paged_attn_tc.cuh"      // generation 2
 
@@ -287,13 +285,6 @@ static int choose_split_tokens(int num_seqs, int nkv, int max_seq_len, int seq_b
     return (int)st;
 }
 
-// SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel (A/B measurements, debugging); default: TMA/wgmma
-// whenever the shape is covered (head_dim 128, block_size 16).
-static int forced_generation() {
-    const char* e = getenv("SLLM_PAGED_ATTN_GEN");      // re-read every call so tests can toggle it
-    return (e && e[0] == '1') ? 1 : (e && e[0] == '2') ? 2 : 0;
-}
-
 template <typename T, int D>
 static int launch_paged(const PagedAttnParams& p, int num_seqs, int max_seq_len, cudaStream_t stream) {
     const size_t smem = (size_t)PA_STAGES * 2 * PA_TILE * D * 2 + (size_t)(p.split_tokens / p.block_size + 2) * sizeof(int32_t);
@@ -359,8 +350,10 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
         p.part_lse = p.part_o + (int64_t)num_decoding_seqs * nq * p.num_splits * head_dim;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (forced_generation() != 1 && tc_paged_supported(head_dim, block_size, nq, nkv, num_blocks, num_layers) &&
-        dtype <= SLLM_BF16) {
+    // SLLM_PAGED_ATTN_GEN=1 forces the cp.async/mma.sync kernel; default: TMA/wgmma whenever the shape is covered (head_dim 128,
+    // block_size 16)
+    const int gen = forced_generation("SLLM_PAGED_ATTN_GEN");
+    if (gen != 1 && tc_paged_supported(head_dim, block_size, nq, nkv, num_blocks, num_layers) && dtype <= SLLM_BF16) {
         TcLaunch a = {};
         a.p.block_table = block_table; a.p.seq_ids = seq_ids; a.p.seq_lens = seq_lens;
         a.p.o = o; a.p.part_o = p.part_o; a.p.part_lse = p.part_lse; a.p.scale_log2e = p.scale_log2e;
@@ -375,7 +368,7 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
                                                                p.num_splits, p.split_tokens, st, "paged_attention(phase 2)")));
         return 0;
     }
-    SLLM_REQUIRE(forced_generation() != 2, "paged_attention: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
+    SLLM_REQUIRE(gen != 2, "paged_attention: SLLM_PAGED_ATTN_GEN=2 but the shape is not covered by the wgmma kernel");
     if (head_dim == 128) { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 128>(p, num_decoding_seqs, max_seq_len, st))); }
     else { SLLM_DISPATCH_DTYPE(dtype, return (launch_paged<T, 64>(p, num_decoding_seqs, max_seq_len, st))); }
     return 0;
@@ -411,7 +404,7 @@ int sllm_paged_attention_verify(const void* q, const void* k_cache, const void* 
                  "paged_attention_verify: bad cache geometry (layer %d of %d)", cur_layer, num_layers);
     cudaStream_t st = (cudaStream_t)stream;
     // SLLM_PAGED_ATTN_GEN=1 forces the paged-prefill kernel below, =2 makes a shape the verify kernel does not serve an error
-    const int gen = forced_generation();
+    const int gen = forced_generation("SLLM_PAGED_ATTN_GEN");
     if (gen != 1 && dtype <= SLLM_BF16 &&
         tc_verify_supported(head_dim, block_size, nq, nkv, max_rows, num_blocks, num_layers, num_tokens)) {
         const int split_tokens = choose_split_tokens(num_seqs, nkv, max_seq_len, 0);

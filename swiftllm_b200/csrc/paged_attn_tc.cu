@@ -21,9 +21,6 @@
 // (entry, kv head, split) item streams its K/V pages once for every row and head of the entry.  Q is one TMA box (64 d, g heads,
 // qrows rows) per d-half over the row-strided packed q: columns of rows past the entry's count hold whatever the box read (the
 // next entry's rows, or zero fill) and are never written.
-#include <mutex>
-#include <unordered_map>
-
 #include "paged_attn_tc.cuh"
 #include "tc_helpers.cuh"
 
@@ -396,79 +393,37 @@ __global__ void __launch_bounds__(TC_THREADS, 1) paged_attn_verify_kernel(const 
 // ------------------------------------------------------------------ host side
 namespace {
 
-struct MapKey {
-    const void* ptr; uint64_t rows; int kind;
-    bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && kind == o.kind; }
-};
-struct MapKeyHash {
-    size_t operator()(const MapKey& k) const {
-        return std::hash<const void*>()(k.ptr) ^ (std::hash<uint64_t>()(k.rows) * 1315423911u) ^ (size_t)k.kind;
-    }
-};
-std::mutex g_map_mutex;
-std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 int g_kv_4d_ok = -1;            // -1 unknown, 0 the driver rejected the permuted-stride 4-D map, 1 usable (a property of the
                                 // driver's tensor-map encoder, identical for every device of the process)
 
-CUtensorMapDataType map_dtype(sllm_dtype_t dt) { return dt == SLLM_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
-
-// kind 0: 2-D [rows, 128] map with (64 x 16) boxes; kind 1: 4-D page map (64 d | 8 tok | 2 halves | rows/8), box (64,8,2,2);
-// kind 2: q as (128 d | nq heads | rows) with `q_row_stride` elements between rows, box (64, box_heads, box_rows)
-bool encode_map(CUtensorMap* out, const void* ptr, uint64_t rows, int kind, sllm_dtype_t dt, int nq = 0, int64_t q_row_stride = 0,
-                int box_heads = 0, int box_rows = 0) {
-    TensorMapEncodeFn enc = get_tensor_map_encoder();
-    if (!enc) return false;
-    CUresult r;
-    if (kind == 0) {
-        cuuint64_t dims[2] = {128, rows};
-        cuuint64_t strides[1] = {256};
-        cuuint32_t box[2] = {64, 16}, es[2] = {1, 1};
-        r = enc(out, map_dtype(dt), 2, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    } else if (kind == 2) {
-        cuuint64_t dims[3] = {128, (cuuint64_t)nq, rows};
-        cuuint64_t strides[2] = {256, (cuuint64_t)q_row_stride * 2};
-        cuuint32_t box[3] = {64, (cuuint32_t)box_heads, (cuuint32_t)box_rows}, es[3] = {1, 1, 1};
-        r = enc(out, map_dtype(dt), 3, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    } else {
-        cuuint64_t dims[4] = {64, 8, 2, rows / 8};
-        cuuint64_t strides[3] = {256, 128, 2048};
-        cuuint32_t box[4] = {64, 8, 2, 2}, es[4] = {1, 1, 1, 1};
-        r = enc(out, map_dtype(dt), 4, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
-    return r == CUDA_SUCCESS;
-}
-
-// K / V cache maps: a cache tensor keeps its address, so its map is encoded once
-bool get_map(CUtensorMap* out, const void* ptr, uint64_t rows, int kind, sllm_dtype_t dt) {
-    MapKey key{ptr, rows, kind * 2 + (int)dt};
-    {
-        std::lock_guard<std::mutex> lk(g_map_mutex);
-        auto it = g_maps.find(key);
-        if (it != g_maps.end()) { *out = it->second; return true; }
-    }
-    if (!encode_map(out, ptr, rows, kind, dt)) return false;
-    std::lock_guard<std::mutex> lk(g_map_mutex);
-    if (g_maps.size() > 4096) g_maps.clear();
-    g_maps[key] = *out;
-    return true;
-}
-
-// The K and V maps of a launch and, in `p`, the shared-memory layout their boxes produce: the 4-D page map where the driver
-// accepts it, else two 2-D boxes per page.
+// The K and V maps of a launch (cached: a cache tensor keeps its address) and, in `p`, the shared-memory layout their boxes
+// produce: the 4-D page map (64 d | 8 tok | 2 halves | rows / 8) with one (64, 8, 2, 2) box per page where the driver accepts
+// it, else the cache as [rows, 128] with two (64 d x 16 tokens) boxes per page.
 bool kv_maps_and_layout(const TcLaunch& a, CUtensorMap* kmap, CUtensorMap* vmap, TcParams& p) {
     const uint64_t rows = (uint64_t)a.num_blocks * p.num_layers * p.nkv * TC_BS;
     if (g_kv_4d_ok != 0) {
-        bool ok = get_map(kmap, a.k_cache, rows, 1, a.dtype) && get_map(vmap, a.v_cache, rows, 1, a.dtype);
+        const cuuint64_t dims[4] = {64, 8, 2, rows / 8}, strides[3] = {256, 128, 2048};
+        const cuuint32_t box[4] = {64, 8, 2, 2};
+        bool ok = cached_tma_map(kmap, a.k_cache, a.dtype, 4, dims, strides, box) &&
+                  cached_tma_map(vmap, a.v_cache, a.dtype, 4, dims, strides, box);
         if (g_kv_4d_ok < 0) g_kv_4d_ok = ok ? 1 : 0;
     }
-    if (g_kv_4d_ok == 0 && !(get_map(kmap, a.k_cache, rows, 0, a.dtype) && get_map(vmap, a.v_cache, rows, 0, a.dtype))) return false;
+    if (g_kv_4d_ok == 0 && !(cached_rows_map(kmap, a.k_cache, a.dtype, rows, TC_D, TC_D, TC_BS) &&
+                             cached_rows_map(vmap, a.v_cache, a.dtype, rows, TC_D, TC_D, TC_BS)))
+        return false;
     p.tma_4d = g_kv_4d_ok == 1;
     if (p.tma_4d) { p.page_stride = 4096; p.half_stride = 1024; p.k_sbo = 2048; p.v_lbo = 1024; p.v_sbo = 2048; }
     else          { p.page_stride = 2048; p.half_stride = 16384; p.k_sbo = 1024; p.v_lbo = 16384; p.v_sbo = 1024; }
     return true;
+}
+
+// q as (128 d | nq heads | num_tokens rows), rows q_row_stride elements apart, boxes of (64 d, box_heads, box_rows).  q is a
+// transient activation (its address changes from call to call): encoded per launch (host-only, ~1 us), never cached.
+bool encode_q_map(CUtensorMap* out, const TcLaunch& a, uint32_t box_heads, uint32_t box_rows) {
+    const cuuint64_t dims[3] = {TC_D, (cuuint64_t)a.p.nq, (cuuint64_t)a.num_tokens};
+    const cuuint64_t strides[2] = {TC_D * 2, (cuuint64_t)a.q_row_stride * 2};
+    const cuuint32_t box[3] = {64, box_heads, box_rows};
+    return encode_tma_map(out, a.q, a.dtype, 3, dims, strides, box);
 }
 
 }  // namespace
@@ -495,9 +450,7 @@ int launch_paged_tc(const TcLaunch& a) {
     const int g = p.nq / p.nkv;
     CUtensorMap kmap, vmap, qmap;
     SLLM_REQUIRE(kv_maps_and_layout(a, &kmap, &vmap, p), "paged_attention: cuTensorMapEncodeTiled failed for the KV cache");
-    // q is a transient activation (its address changes from call to call): encoded per launch (host-only, ~1 us), never cached
-    SLLM_REQUIRE(encode_map(&qmap, a.q, (uint64_t)a.num_tokens, 2, a.dtype, p.nq, a.q_row_stride, TC_NPAD, 1),
-                 "paged_attention: cuTensorMapEncodeTiled failed for q");
+    SLLM_REQUIRE(encode_q_map(&qmap, a, TC_NPAD, 1), "paged_attention: cuTensorMapEncodeTiled failed for q");
     p.num_items = a.num_seqs * p.nkv * p.num_splits;
     const int grid = p.num_items < a.num_sms ? p.num_items : a.num_sms;
     if (a.dtype == SLLM_F16) {
@@ -521,8 +474,7 @@ int launch_paged_verify_tc(const TcLaunch& a) {
     const int g = p.nq / p.nkv;
     CUtensorMap kmap, vmap, qmap;
     SLLM_REQUIRE(kv_maps_and_layout(a, &kmap, &vmap, p), "paged_attention_verify: cuTensorMapEncodeTiled failed for the KV cache");
-    SLLM_REQUIRE(encode_map(&qmap, a.q, (uint64_t)a.num_tokens, 2, a.dtype, p.nq, a.q_row_stride, g, p.qrows),
-                 "paged_attention_verify: cuTensorMapEncodeTiled failed for q");
+    SLLM_REQUIRE(encode_q_map(&qmap, a, g, p.qrows), "paged_attention_verify: cuTensorMapEncodeTiled failed for q");
     p.num_items = a.num_seqs * p.nkv * p.num_splits;
     const int grid = p.num_items < a.num_sms ? p.num_items : a.num_sms;
     const int cols = g * p.qrows;

@@ -1,6 +1,6 @@
-// Causal varlen prefill attention, generation 1 kernel (cp.async double buffering + mma.sync), shared by
-// prefill_attn.cu (packed k/v of the batch: the reference's contract) and prefill_attn_paged.cu (chunked prefill:
-// k/v gathered from the paged KV cache through the block table).
+// Causal varlen prefill attention, generation 1 kernel (cp.async double buffering + mma.sync).  Launched by
+// prefill_attn.cu for packed k/v of the batch (PAGED = false: the reference's contract) and for chunked prefill
+// (PAGED = true: k/v gathered from the paged KV cache through the block table).
 //
 // Reference: swiftllm/worker/kernels/prefill_attn.py:9-139 (the Triton kernel) and the flash_attn_varlen_func
 // call that stands in for it at swiftllm/worker/layers/transformer_layer.py:86-96.  Numerics follow

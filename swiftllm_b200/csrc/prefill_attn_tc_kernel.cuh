@@ -1,6 +1,6 @@
 // Causal varlen prefill attention, generation 2 kernel: TMA + wgmma, two consumer warpgroups per CTA (sm_90a).
-// Shared by prefill_attn_tc.cu (packed k/v of the batch) and prefill_attn_paged.cu (chunked prefill: K/V pages gathered
-// from the KV cache through the block table).
+// Launched by prefill_attn.cu for packed k/v of the batch (PAGED = false) and for chunked prefill (PAGED = true: K/V pages
+// gathered from the KV cache through the block table).
 //
 // Reference being replaced: swiftllm/worker/kernels/prefill_attn.py:9-139 and the flash_attn_varlen_func call at
 // swiftllm/worker/layers/transformer_layer.py:86-96.  head_dim 128, fp16/bf16; numerics per SURVEY.md Appendix A6
@@ -265,8 +265,5 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
         }
     }
 }
-
-// host (prefill_attn_tc.cu): cached cuTensorMapEncodeTiled of a [rows, cols] 16-bit tensor, boxes of (64 cols x box_rows)
-bool pt_map(CUtensorMap* out, const void* ptr, uint64_t rows, int cols, int64_t row_stride, int box_rows, sllm_dtype_t dt);
 
 }  // namespace sllm

@@ -181,5 +181,21 @@ typedef CUresult (*TensorMapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint3
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 TensorMapEncodeFn get_tensor_map_encoder();     // nullptr if unavailable (host.cu)
 
+// Every tensor map of the library (host.cu): 16-bit elements, SWIZZLE_128B, L2_256B promotion, no OOB fill, unit element
+// strides.  dims[0] is the contiguous dimension; byte_strides[i] is the distance between consecutive indices of dims[i + 1].
+// False if the encoder is unavailable or rejects the geometry.
+bool encode_tma_map(CUtensorMap* out, const void* ptr, sllm_dtype_t dt, int rank, const cuuint64_t* dims,
+                    const cuuint64_t* byte_strides, const cuuint32_t* box);
+// The same, memoised on all arguments (a KV cache keeps its address, so its maps are encoded once)
+bool cached_tma_map(CUtensorMap* out, const void* ptr, sllm_dtype_t dt, int rank, const cuuint64_t* dims,
+                    const cuuint64_t* byte_strides, const cuuint32_t* box);
+// A [rows, cols] tensor with rows `row_stride` elements apart, boxes of (64 cols x box_rows), cached
+inline bool cached_rows_map(CUtensorMap* out, const void* ptr, sllm_dtype_t dt, uint64_t rows, uint64_t cols, int64_t row_stride,
+                            uint32_t box_rows) {
+    const cuuint64_t dims[2] = {cols, rows}, strides[1] = {(cuuint64_t)row_stride * 2};
+    const cuuint32_t box[2] = {64, box_rows};
+    return cached_tma_map(out, ptr, dt, 2, dims, strides, box);
+}
+
 }  // namespace tc
 }  // namespace sllm
