@@ -94,6 +94,10 @@ int sllm_paged_attention(const void* q, const void* k_cache, const void* v_cache
                          int seq_block_size, int cur_layer, int num_layers, int num_q_heads, int num_kv_heads,
                          int block_size, int head_dim, int max_blocks_per_seq, int64_t num_blocks,
                          int64_t q_row_stride, sllm_dtype_t dtype, sllm_stream_t stream);
+/* Rank of the KV-cache tensor map the next sm_90a decode or verification launch uses: 4 (one box per 16-token page) where the
+ * driver accepts the permuted-stride 4-D map, 2 (the cache as [rows, 128], two boxes per page) where it does not or where
+ * SLLM_PAGED_ATTN_KV_MAP=2d is set (read on every launch); -1 while no launch has asked the driver yet. */
+int sllm_paged_attention_kv_map_rank(void);
 
 /* ---- Prefill attention: swiftllm/worker/kernels/prefill_attn.py:102-139 (prefill_attention) and the
  * flash_attn_varlen_func call it stands for (swiftllm/worker/layers/transformer_layer.py:86-96).

@@ -37,6 +37,7 @@ SIGNATURES = {
     "sllm_paged_attention_verify_workspace_bytes": (_L, [_I, _L, _I, _I, _I, _I]),
     "sllm_paged_attention_verify": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _F, _I, _I, _I, _L, _I, _I, _I, _I, _I, _I, _I,
                                          _L, _L, _I, _P]),
+    "sllm_paged_attention_kv_map_rank": (_I, []),
     "sllm_set_block_table_and_num_seq_alloc_blocks": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
     "sllm_truncate_blocks_for_seqs": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "sllm_unset_block_table_and_num_seq_alloc_blocks": (_I, [_P, _P, _P, _P, _I, _I, _P]),

@@ -396,22 +396,31 @@ namespace {
 int g_kv_4d_ok = -1;            // -1 unknown, 0 the driver rejected the permuted-stride 4-D map, 1 usable (a property of the
                                 // driver's tensor-map encoder, identical for every device of the process)
 
-// The K and V maps of a launch (cached: a cache tensor keeps its address) and, in `p`, the shared-memory layout their boxes
-// produce: the 4-D page map (64 d | 8 tok | 2 halves | rows / 8) with one (64, 8, 2, 2) box per page where the driver accepts
-// it, else the cache as [rows, 128] with two (64 d x 16 tokens) boxes per page.
+// SLLM_PAGED_ATTN_KV_MAP=2d: the [rows, 128] map even where the driver accepts the 4-D one, so the layout a driver without the
+// 4-D map gets can be run and checked anywhere.  Read on every launch; the driver probe (g_kv_4d_ok) is left as it is.
+bool kv_map_forced_2d() {
+    const char* e = getenv("SLLM_PAGED_ATTN_KV_MAP");
+    return e && strcmp(e, "2d") == 0;
+}
+
+// The K and V maps of a launch (cached by every argument: a cache tensor keeps its address, and both layouts of one cache can be
+// cached at once) and, in `p`, the shared-memory layout their boxes produce: the 4-D page map (64 d | 8 tok | 2 halves |
+// rows / 8) with one (64, 8, 2, 2) box per page where the driver accepts it, else the cache as [rows, 128] with two
+// (64 d x 16 tokens) boxes per page.
 bool kv_maps_and_layout(const TcLaunch& a, CUtensorMap* kmap, CUtensorMap* vmap, TcParams& p) {
     const uint64_t rows = (uint64_t)a.num_blocks * p.num_layers * p.nkv * TC_BS;
-    if (g_kv_4d_ok != 0) {
+    bool ok_4d = false;
+    if (!kv_map_forced_2d() && g_kv_4d_ok != 0) {
         const cuuint64_t dims[4] = {64, 8, 2, rows / 8}, strides[3] = {256, 128, 2048};
         const cuuint32_t box[4] = {64, 8, 2, 2};
-        bool ok = cached_tma_map(kmap, a.k_cache, a.dtype, 4, dims, strides, box) &&
-                  cached_tma_map(vmap, a.v_cache, a.dtype, 4, dims, strides, box);
-        if (g_kv_4d_ok < 0) g_kv_4d_ok = ok ? 1 : 0;
+        ok_4d = cached_tma_map(kmap, a.k_cache, a.dtype, 4, dims, strides, box) &&
+                cached_tma_map(vmap, a.v_cache, a.dtype, 4, dims, strides, box);
+        if (g_kv_4d_ok < 0) g_kv_4d_ok = ok_4d ? 1 : 0;
     }
-    if (g_kv_4d_ok == 0 && !(cached_rows_map(kmap, a.k_cache, a.dtype, rows, TC_D, TC_D, TC_BS) &&
-                             cached_rows_map(vmap, a.v_cache, a.dtype, rows, TC_D, TC_D, TC_BS)))
+    if (!ok_4d && !(cached_rows_map(kmap, a.k_cache, a.dtype, rows, TC_D, TC_D, TC_BS) &&
+                    cached_rows_map(vmap, a.v_cache, a.dtype, rows, TC_D, TC_D, TC_BS)))
         return false;
-    p.tma_4d = g_kv_4d_ok == 1;
+    p.tma_4d = ok_4d;
     if (p.tma_4d) { p.page_stride = 4096; p.half_stride = 1024; p.k_sbo = 2048; p.v_lbo = 1024; p.v_sbo = 2048; }
     else          { p.page_stride = 2048; p.half_stride = 16384; p.k_sbo = 1024; p.v_lbo = 16384; p.v_sbo = 1024; }
     return true;
@@ -492,3 +501,8 @@ int launch_paged_verify_tc(const TcLaunch& a) {
 #undef SLLM_TC_LAUNCH
 
 }  // namespace sllm
+
+extern "C" int sllm_paged_attention_kv_map_rank(void) {
+    if (sllm::kv_map_forced_2d()) return 2;
+    return sllm::g_kv_4d_ok < 0 ? -1 : sllm::g_kv_4d_ok == 1 ? 4 : 2;
+}
