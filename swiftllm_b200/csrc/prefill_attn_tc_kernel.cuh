@@ -35,6 +35,7 @@ constexpr float PT_RESCALE_THRESHOLD = 8.0f;          // log2 units
 struct PtBarriers {
     uint64_t q_full;
     uint64_t k_full[PT_STAGES], k_empty[PT_STAGES], v_full[PT_STAGES], v_empty[PT_STAGES];
+    uint64_t v_tail;                      // packed only: the TMA of a last V step that ends past the sequence completes here
 };
 
 struct PtParams {
@@ -92,6 +93,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
             mbar_init(smem_u32(&bars->k_full[i]), 1); mbar_init(smem_u32(&bars->k_empty[i]), 256);
             mbar_init(smem_u32(&bars->v_full[i]), 1); mbar_init(smem_u32(&bars->v_empty[i]), 256);
         }
+        if constexpr (!PAGED) mbar_init(smem_u32(&bars->v_tail), 1);
         mbar_fence_init();
         tma_prefetch_desc(&qmap); tma_prefetch_desc(&kmap); tma_prefetch_desc(&vmap);
     }
@@ -150,14 +152,35 @@ __global__ void __launch_bounds__(PT_THREADS, 1) prefill_attn_tc_kernel(const __
         // =========================================================== TMA producer: the V tiles (independent of K's progress)
         if constexpr (PAGED) {
             paged_producer(vmap, v_sm, bars->v_full, bars->v_empty);
-        } else if (lane == 0) {
-            for (int j = 0; j < nkt; j++) {
-                const int st = j % PT_STAGES;
-                mbar_wait(smem_u32(&bars->v_empty[st]), ((j / PT_STAGES) & 1) ^ 1);
-                const uint32_t vb = smem_u32(&bars->v_full[st]);
-                mbar_arrive_expect_tx(vb, PT_KV_BYTES);
-                tma_load_2d(smem_u32(v_sm + st * PT_KV_BYTES), &vmap, vb, kvh * PT_D, tok0 + j * PT_BK);
-                tma_load_2d(smem_u32(v_sm + st * PT_KV_BYTES + PT_KV_BYTES / 2), &vmap, vb, kvh * PT_D + 64, tok0 + j * PT_BK);
+        } else {
+            // The tail step's box runs past the sequence into the next prompt's rows (or rows past the batch).  Their P is
+            // exactly 0, but 0 x Inf and 0 x NaN are NaN, so a non-finite V there would leak into this prompt.  That step's
+            // TMA therefore completes on v_tail instead; the warp zeroes rows valid..63 and only then completes v_full with a
+            // plain arrive, so the consumers are unchanged.  Row r of a d-half is the 128-byte line r (SWIZZLE_128B only
+            // permutes the 16-byte chunks within a line).
+            const int valid = kvlen - (nkt - 1) * PT_BK;        // rows of the last step inside the sequence
+            if (lane == 0) {
+                for (int j = 0; j < nkt; j++) {
+                    const int st = j % PT_STAGES;
+                    mbar_wait(smem_u32(&bars->v_empty[st]), ((j / PT_STAGES) & 1) ^ 1);
+                    const uint32_t vb = smem_u32(j == nkt - 1 && valid < PT_BK ? &bars->v_tail : &bars->v_full[st]);
+                    mbar_arrive_expect_tx(vb, PT_KV_BYTES);
+                    tma_load_2d(smem_u32(v_sm + st * PT_KV_BYTES), &vmap, vb, kvh * PT_D, tok0 + j * PT_BK);
+                    tma_load_2d(smem_u32(v_sm + st * PT_KV_BYTES + PT_KV_BYTES / 2), &vmap, vb, kvh * PT_D + 64, tok0 + j * PT_BK);
+                }
+            }
+            if (valid < PT_BK) {
+                const int st = (nkt - 1) % PT_STAGES;
+                __syncwarp();                                      // lanes 1-31 sleep here while lane 0 streams
+                mbar_wait(smem_u32(&bars->v_tail), 0);            // used once per CTA
+                uint8_t* tile = v_sm + st * PT_KV_BYTES;
+                for (int i = lane; i < 2 * (PT_BK - valid) * 8; i += 32) {         // 8 chunks of 16 B per row and d-half
+                    const int h = i / ((PT_BK - valid) * 8), r = valid + (i >> 3) % (PT_BK - valid);
+                    *reinterpret_cast<uint4*>(tile + h * (PT_KV_BYTES / 2) + r * 128 + (i & 7) * 16) = make_uint4(0, 0, 0, 0);
+                }
+                fence_proxy_async();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(smem_u32(&bars->v_full[st]));
             }
         }
     } else if (warp >= 4) {
