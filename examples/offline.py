@@ -9,6 +9,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --cuda-graph       replay decode steps from CUDA graphs
     ... --temperature 0.8 --top-p 0.95 [--top-k 50] [--seed 1]    sample instead of greedy decoding
     ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
+    ... --prompt-logprobs 3    print each prompt's perplexity and the 3 most likely tokens at its first positions
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
     ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
@@ -21,6 +22,7 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import swiftllm_b200  # noqa: E402
@@ -37,12 +39,15 @@ def prompt_lookup(tokens: list, k: int, max_ngram: int = 3) -> list:
     return []
 
 
-def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0, n: int = 1):
+def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0, n: int = 1,
+             prompt_logs=None):
     """Generation for a batch of prompts (sequence i uses block-table row i), greedy unless `params` (one
     swiftllm_b200.SamplingParams for every sequence) is given.  chunk > 0: the prompts are prefilled `chunk` tokens at a time
     through the paged cache.  speculate > 0: decoding verifies up to that many prompt-lookup drafts per step
     (forward_speculative); the tokens are the ones plain decoding returns.  Returns (token lists, prefill seconds, decode seconds).
-    With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token.
+    With params.logprobs set, logs[i] (a list per sequence) receives the TokenLogprobs of every generated token.  With
+    params.prompt_logprobs set, prompt_logs[i] (a list per prompt) receives the PromptLogprobs of each of its prefill calls: with
+    chunks, each call passes the next chunk's first token, so together they score positions 1 .. len - 1.
 
     n > 1: n samples per prompt.  Each prompt is prefilled once into row i; rows len(input_ids) + i * (n - 1) + j (j < n - 1)
     fork its first len - 1 tokens (fork_seqs: the full blocks are shared) and draw their own first token from the last prompt
@@ -56,27 +61,34 @@ def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, log
     row_params = [params] * P + [params if params is None or params.seed is None else
                                  dataclasses.replace(params, seed=(params.seed + k) % 2 ** 64) for _, _, k in kids]
     sp = (lambda rows: None) if params is None else (lambda rows: [row_params[i] for i in rows])
-    want_lp = params is not None and params.logprobs is not None
+    want_lp = params is not None and (params.logprobs is not None or params.prompt_logprobs is not None)
     logs = logs if logs is not None else [[] for _ in range(P * n)]
+    prompt_logs = prompt_logs if prompt_logs is not None else [[] for _ in range(P)]
 
-    def step(*args, **kw):
+    def step(*args, prompt_next_ids_list=None, **kw):
         if not want_lp:
             return model.forward(*args, **kw)
-        return model.forward_with_logprobs(*args, **kw)
+        return model.forward_with_logprobs(*args, prompt_next_ids_list=prompt_next_ids_list, **kw)
     t0 = time.perf_counter()
     if chunk > 0:                      # every call carries the next chunk of each unfinished prompt
         done = [0] * len(input_ids)
         last = [None] * len(input_ids)
         while any(d < len(p) for d, p in zip(done, input_ids)):
             live = [i for i in seq_ids if done[i] < len(input_ids[i])]
+            nxt = [input_ids[i][done[i] + chunk] if done[i] + chunk < len(input_ids[i]) else None for i in live]
             toks = step([input_ids[i][done[i]:done[i] + chunk] for i in live], live, [],
-                        prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(live))
+                        prefill_prefix_lens_list=[done[i] for i in live], sampling_params_list=sp(live), prompt_next_ids_list=nxt)
             for i, t in zip(live, toks):
+                if want_lp and t.prompt is not None:
+                    prompt_logs[i].append(t.prompt)
                 done[i] = min(len(input_ids[i]), done[i] + chunk)
                 if done[i] == len(input_ids[i]):
                     last[i] = t             # the token sampled after the LAST chunk is the first generated token
     else:
         last = step(input_ids, seq_ids, [], sampling_params_list=sp(seq_ids))
+        for i, t in enumerate(last if want_lp else []):
+            if t.prompt is not None:
+                prompt_logs[i].append(t.prompt)
     if kids:
         rows = [r for _, r, _ in kids]
         model.fork_seqs([i for i, _, _ in kids], rows, [len(input_ids[i]) - 1 for i, _, _ in kids])
@@ -129,6 +141,8 @@ def main():
     ap.add_argument("--top-p", type=float, default=1.0, help="keep the smallest set of tokens with this much mass (1 = off)")
     ap.add_argument("--seed", type=int, default=None, help="sampling seed (default: a fresh one per step from the engine's generator)")
     ap.add_argument("--logprobs", type=int, default=None, help="print each token's log-probability and the N most likely tokens (0..20)")
+    ap.add_argument("--prompt-logprobs", type=int, default=None,
+                    help="print each prompt's perplexity and the N most likely tokens at its first positions (0..20)")
     ap.add_argument("--repetition-penalty", type=float, default=1.0, help="divide / multiply the logits of seen tokens (1 = off)")
     ap.add_argument("--frequency-penalty", type=float, default=0.0, help="subtract this times each token's output count (0 = off)")
     ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
@@ -139,9 +153,9 @@ def main():
         ap.error("--n takes a positive number of samples")
     if not 0 <= args.speculate <= 7:
         ap.error("--speculate takes 0..7 drafts")
-    if args.speculate and (args.logprobs is not None or args.repetition_penalty != 1.0 or args.frequency_penalty != 0.0
+    if args.speculate and (args.logprobs is not None or args.prompt_logprobs is not None or args.repetition_penalty != 1.0 or args.frequency_penalty != 0.0
                            or args.presence_penalty != 0.0):
-        ap.error("--speculate does not combine with --logprobs or penalties")
+        ap.error("--speculate does not combine with --logprobs, --prompt-logprobs or penalties")
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
                                     num_cpu_blocks=0, max_seqs_in_block_table=128, max_blocks_per_seq=2048, max_batch_size=16,
@@ -170,19 +184,31 @@ def main():
     print(f"{num_blocks} KV blocks; model ready in {time.perf_counter() - t0:.1f} s")
 
     params = swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs,
+                                          prompt_logprobs=args.prompt_logprobs,
                                           repetition_penalty=args.repetition_penalty, frequency_penalty=args.frequency_penalty,
                                           presence_penalty=args.presence_penalty)
-    if args.temperature == 0 and args.logprobs is None and not params.has_penalties():
+    if args.temperature == 0 and args.logprobs is None and args.prompt_logprobs is None and not params.has_penalties():
         params = None
     logs = [[] for _ in range(len(input_ids) * args.n)]
-    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs, args.speculate, args.n)
+    prompt_logs = [[] for _ in input_ids]
+    outputs, t_prefill, t_decode = generate(model, input_ids, args.new_tokens, args.chunk, params, logs, args.speculate, args.n,
+                                            prompt_logs)
+    for i, pls in enumerate(prompt_logs if args.prompt_logprobs is not None else []):
+        lp = np.concatenate([pl.logprobs for pl in pls]) if pls else np.zeros((0,))
+        ppl = float(np.exp(-lp.astype(np.float64).mean())) if lp.size else float("nan")
+        print(f"prompt {i}: {lp.size} scored tokens, perplexity {ppl:.3f}")
+        for pl in pls[:1]:
+            for j in range(min(4, len(pl.token_ids))):
+                top = ", ".join(f"{show([int(t)])!r}:{float(v):.3f}" for t, v in zip(pl.top_ids[j], pl.top_logprobs[j]))
+                print(f"    pos {pl.first_position + j} {show([int(pl.token_ids[j])])!r} {pl.logprobs[j]:.4f} "
+                      f"rank {pl.ranks[j]}   top [{top}]")
     seq_ids = list(range(len(outputs)))
     # rows of prompt i: i, then its forks
     rows = [k for i in range(len(input_ids)) for k in [i] + [len(input_ids) + i * (args.n - 1) + j for j in range(args.n - 1)]]
     for k in rows:
         p, o, lg = input_ids[k if k < len(input_ids) else (k - len(input_ids)) // (args.n - 1)], outputs[k], logs[k]
         print(f"[{len(p)} prompt tokens] -> {show(o)}")
-        for r in lg:      # log-probabilities of the raw model distribution (before penalties, temperature / top-k / top-p)
+        for r in lg if args.logprobs is not None else []:      # log-probabilities of the raw model distribution (before penalties, temperature / top-k / top-p)
             top = ", ".join(f"{show([t])!r}:{lp:.3f}" for t, lp in r.top)
             print(f"    {show([r.token])!r} {r.logprob:.4f}   top [{top}]")
     print(f"prefill {t_prefill * 1e3:.1f} ms ({sum(map(len, input_ids)) / t_prefill:.0f} tok/s), "

@@ -297,6 +297,18 @@ int sllm_token_logprobs(const void* logits, int64_t num_rows, int vocab_size, in
                         const int64_t* token_ids, int top_n, float* out_token_logprob, int32_t* out_top_ids,
                         float* out_top_logprobs, sllm_dtype_t dtype, sllm_stream_t stream);
 
+/* ---- Prompt log-probabilities (new): sllm_token_logprobs' values for many rows at once (every row of a prefill), plus ranks.
+ * target_ids int32 [num_rows]: out_logprob fp32 [num_rows] = logprob(target_ids[i]), bit-identical to sllm_token_logprobs on
+ * the same row; out_rank int32 [num_rows] = 1 + the number of ids whose logit is strictly greater (-0 == +0; NaN and inf in the
+ * order of sllm_token_logprobs' top-N), so a greedy token has rank 1; an id outside [0, vocab_size) gives NaN and rank -1.
+ * top_n in [0, 20]: out_top_ids / out_top_logprobs [num_rows, top_n] as in sllm_token_logprobs.  One CTA per row, no clusters.
+ * Deterministic: a row's outputs depend on its logits and target only.  Rejected before launch: unknown dtype, vocab_size
+ * outside [1, 2^24], top_n outside [0, 20], a row stride below vocab_size, num_rows outside [0, 2^24], null pointers
+ * (out_top_* may be NULL when top_n is 0). */
+int sllm_prompt_logprobs(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                         const int32_t* target_ids, int top_n, float* out_logprob, int32_t* out_rank, int32_t* out_top_ids,
+                         float* out_top_logprobs, sllm_dtype_t dtype, sllm_stream_t stream);
+
 /* ---- Repetition / frequency / presence penalties (new; the reference has no sampling controls), IN PLACE on logits laid out
  * as in sllm_sample_tokens (a vocabulary shard with vocab_offset works).  Per-row DEVICE arrays [num_rows]:
  * repetition_penalty, frequency_penalty, presence_penalty (a row with 1, 0, 0 is skipped: nothing read, recorded or modified),

@@ -26,24 +26,6 @@ namespace {
 
 constexpr int kMaxTopN = 20;
 
-// key_of of +inf and -inf: keys above the first are NaN / +inf, keys below the second are NaN
-template <typename T> struct InfKeys;
-template <> struct InfKeys<__half> { static constexpr uint32_t pos = 0xfc00u, neg = 0x03ffu; };
-template <> struct InfKeys<__nv_bfloat16> { static constexpr uint32_t pos = 0xff80u, neg = 0x007fu; };
-
-__device__ unsigned long long block_sum_u64(unsigned long long v, unsigned long long* scratch) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0) scratch[warp] = v;
-    __syncthreads();
-    v = lane < (int)(blockDim.x >> 5) ? scratch[lane] : 0ull;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 template <typename T>
 __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict__ logits, int64_t row_stride, int V, int slice,
                                                             const int64_t* __restrict__ token_ids, int top_n,

@@ -1,6 +1,7 @@
 // Device helpers shared by the kernels that work on whole vocabulary rows with one thread-block cluster per row
 // (sampling.cu, logprobs.cu): the order-preserving 16-bit keys, the cluster geometry, and the exact two-byte radix select over
-// per-CTA histograms merged through distributed shared memory.
+// per-CTA histograms merged through distributed shared memory.  prompt_logprobs.cu (one CTA per row) uses the keys and the
+// block reductions.
 #pragma once
 #include <cooperative_groups.h>
 #include <type_traits>
@@ -25,6 +26,25 @@ template <typename T> __device__ __forceinline__ float value_of(uint32_t key) {
     const uint16_t bits = (key & 0x8000u) ? (uint16_t)(key ^ 0x8000u) : (uint16_t)(~key & 0xffffu);
     if constexpr (std::is_same<T, __half>::value) return __half2float(__ushort_as_half(bits));
     else return __uint_as_float((uint32_t)bits << 16);
+}
+
+// key_of of +inf and -inf: keys above the first are NaN / +inf, keys below the second are NaN
+template <typename T> struct InfKeys;
+template <> struct InfKeys<__half> { static constexpr uint32_t pos = 0xfc00u, neg = 0x03ffu; };
+template <> struct InfKeys<__nv_bfloat16> { static constexpr uint32_t pos = 0xff80u, neg = 0x007fu; };
+
+// Block-wide sum of a u64 (all threads get it).
+__device__ unsigned long long block_sum_u64(unsigned long long v, unsigned long long* scratch) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __syncthreads();
+    if (lane == 0) scratch[warp] = v;
+    __syncthreads();
+    v = lane < (int)(blockDim.x >> 5) ? scratch[lane] : 0ull;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
 }
 
 // Block-wide max of a u64 (all threads get it).

@@ -19,6 +19,10 @@ class SamplingParams:
     top-N alternatives.  They are log_softmax of the raw logits - the model's distribution before penalties, temperature, top-k and
     top-p; a penalised greedy token therefore need not be top[0].  forward / forward_async ignore the field.
 
+    prompt_logprobs (LlamaModel.forward_with_logprobs, prefill entries): None returns none, 0 the log-probability and rank of
+    every scored prompt token, 1..20 also its top-N alternatives (PromptLogprobs), of the same raw distribution.  It changes
+    neither the staged sampling words nor the tokens; forward / forward_async / forward_speculative ignore it.
+
     Penalties (csrc/penalties.cu; the order and formulas of vLLM), applied to the logits before greedy argmax or sampling, in fp32:
     repetition_penalty r (1: off) divides a positive logit / multiplies a non-positive one of every token seen in the prompt or
     the output; then frequency_penalty f and presence_penalty p (0: off) subtract f * count + p from every token that occurs
@@ -29,6 +33,7 @@ class SamplingParams:
     top_p: float = 1.0
     seed: Optional[int] = None
     logprobs: Optional[int] = None
+    prompt_logprobs: Optional[int] = None
     repetition_penalty: float = 1.0
     frequency_penalty: float = 0.0
     presence_penalty: float = 0.0
@@ -43,9 +48,10 @@ class SamplingParams:
         if self.seed is not None and (isinstance(self.seed, bool) or not isinstance(self.seed, (int, np.integer))
                                       or not 0 <= self.seed < 2 ** 64):
             raise ValueError(f"seed must be None or an integer in [0, 2^64), got {self.seed!r}")
-        if self.logprobs is not None and (isinstance(self.logprobs, bool) or not isinstance(self.logprobs, (int, np.integer))
-                                          or not 0 <= self.logprobs <= MAX_LOGPROBS):
-            raise ValueError(f"logprobs must be None or an integer in [0, {MAX_LOGPROBS}], got {self.logprobs!r}")
+        for name in ("logprobs", "prompt_logprobs"):
+            v = getattr(self, name)
+            if v is not None and (isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= v <= MAX_LOGPROBS):
+                raise ValueError(f"{name} must be None or an integer in [0, {MAX_LOGPROBS}], got {v!r}")
         if not (_is_real(self.repetition_penalty) and math.isfinite(self.repetition_penalty) and self.repetition_penalty > 0):
             raise ValueError(f"repetition_penalty must be a finite number > 0, got {self.repetition_penalty!r}")
         for name in ("frequency_penalty", "presence_penalty"):
@@ -61,18 +67,40 @@ def _is_real(v) -> bool:
     return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool)
 
 
+class PromptLogprobs(NamedTuple):
+    """The scored prompt tokens of one prefill entry (SamplingParams.prompt_logprobs).  An entry at prefix p holding tokens
+    x_p .. x_{p+n-1} scores x_{p+1} .. x_{p+n-1}, and the next prompt token when the caller passes it: k = n - 1 (+ 1) tokens at
+    positions first_position = p + 1 onwards (position 0 is never scored).  Row j: token_ids[j], its log-probability under the
+    raw model distribution given the tokens before it, its rank (1 + the number of ids with a larger logit; 1 for the greedy
+    token) and the N most likely ids with their log-probabilities, ordered by (logprob desc, id asc)."""
+    first_position: int
+    token_ids: np.ndarray           # int64 [k]
+    logprobs: np.ndarray            # float32 [k]
+    ranks: np.ndarray               # int32 [k]
+    top_ids: np.ndarray             # int32 [k, N]
+    top_logprobs: np.ndarray        # float32 [k, N]
+
+
 class TokenLogprobs(NamedTuple):
     """One batch entry of LlamaModel.forward_with_logprobs.  logprob: log-probability of `token` under the raw model
     distribution (log_softmax of the logits); top: [(token id, logprob)] of the N most likely tokens, most likely first, ties
-    broken by the smaller id (the empty list for logprobs=0).  Both None when the entry did not ask."""
+    broken by the smaller id (the empty list for logprobs=0).  Both None when the entry did not ask.  prompt: the entry's
+    PromptLogprobs when it is a prefill entry with SamplingParams.prompt_logprobs set, else None."""
     token: int
     logprob: Optional[float] = None
     top: Optional[list] = None
+    prompt: Optional[PromptLogprobs] = None
 
 
 def logprobs_top_n(params_list: Optional[list]) -> Optional[int]:
     """The per-launch N: the largest `logprobs` of the (validated) list, None when no entry asks."""
     asked = [int(sp.logprobs) for sp in params_list or [] if sp.logprobs is not None]
+    return max(asked) if asked else None
+
+
+def prompt_logprobs_top_n(params_list: Optional[list]) -> Optional[int]:
+    """The per-launch N of the prompt rows: the largest `prompt_logprobs` of the (validated) list, None when no entry asks."""
+    asked = [int(sp.prompt_logprobs) for sp in params_list or [] if sp.prompt_logprobs is not None]
     return max(asked) if asked else None
 
 

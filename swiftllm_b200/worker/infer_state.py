@@ -57,6 +57,22 @@ class LlamaInferState:
     # Top-N of the step's log-probabilities (the largest SamplingParams.logprobs of the batch); None = no log-probabilities,
     # and the post layer returns the token tensor alone
     logprobs: Optional[int] = None
+    # Prompt log-probabilities (SamplingParams.prompt_logprobs): the prefill rows to score; None = none, and the post layer
+    # returns what it returned before
+    prompt_logprobs: Optional["PromptLogprobsState"] = None
+
+
+@dataclasses.dataclass
+class PromptLogprobsState:
+    # host ints, one per asking entry with rows to score, in batch order: (first row in the activation matrix, token count n,
+    # id of the prompt token after the entry or None).  Its rows are [first, first + n - 1), plus the last one with a next id;
+    # row r scores input_ids[r + 1], the last row the next id.  The device tensors are built by the post layer after the layers,
+    # so the prompt part allocates nothing while the forward's activations are live.
+    pieces: list
+    num_rows: int                   # K, the rows to score
+    input_ids: torch.Tensor         # [num_tokens] int32 the step's staged input ids
+    top_n: int                      # the largest prompt_logprobs of the asking entries
+    block_rows: int                 # rows per lm_head + log-probability block (bounds the step's extra memory)
 
 
 @dataclasses.dataclass

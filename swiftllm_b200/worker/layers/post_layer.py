@@ -18,13 +18,18 @@ Addition (penalties, csrc/penalties.cu): when some row carries repetition / freq
 the logits the token is chosen from are penalised first (a copy when log-probabilities are asked for: they stay those of the raw
 logits) and the step's tokens are recorded in the token pages.  With a sharded lm_head the pair-merge path penalises each rank's
 shard (vocab_offset) before its local choice; the gather path penalises the gathered full rows on every rank.  Every rank records
-the same tokens in its own pages."""
+the same tokens in its own pages.
+
+Addition (prompt log-probabilities, csrc/prompt_logprobs.cu): when the step scores prompt rows (infer_state.prompt_logprobs),
+the last-row path above runs first, unchanged; then the prompt rows go through the final RMSNorm, lm_head (gathered when
+sharded, as above) and the prompt kernel in blocks of `block_rows` rows, written into slices of preallocated outputs, and the
+layer returns (what the last-row path returned, (logprobs, ranks, top ids, top logprobs) of the rows)."""
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.linear import linear
-from swiftllm_b200.worker.kernels.logprobs import token_logprobs
+from swiftllm_b200.worker.kernels.logprobs import prompt_logprobs, token_logprobs
 from swiftllm_b200.worker.kernels.penalties import apply_penalties
 from swiftllm_b200.worker.kernels.rmsnorm import rmsnorm_inplace
 from swiftllm_b200.worker.kernels.sampling import sample_tokens
@@ -48,11 +53,48 @@ class LlamaPostLayer:
         self.sharded = bool(getattr(weights, "lm_head_sharded", False))
         assert model_config.vocab_size < (1 << 24) or not self.sharded
         self.last_logits = None     # kept for parity tests (the reference discards them)
+        self.last_prompt_logits = None      # the scored prompt rows' logits, likewise
         self.keep_logits = False
 
-    def forward(self, input_embds: torch.Tensor, infer_state: LlamaInferState, already_normed: bool = False) -> torch.Tensor:
+    def forward(self, input_embds: torch.Tensor, infer_state: LlamaInferState, already_normed: bool = False):
         """`already_normed`: input_embds rows are rmsnorm(final residual) already (TP fused-exchange path; RMSNorm is
         row-wise, so normalising before or after the last-token gather is the same computation)."""
+        out = self._last_rows(input_embds, infer_state, already_normed)
+        if infer_state.prompt_logprobs is None:
+            return out
+        return out, self._prompt_rows(input_embds, infer_state.prompt_logprobs, already_normed)
+
+    def _prompt_rows(self, input_embds: torch.Tensor, st, already_normed: bool):
+        """(logprob fp32 [K], rank int32 [K], top ids int32 [K, N], top logprobs fp32 [K, N]) of the rows of st.pieces, computed
+        st.block_rows rows at a time so the logits block stays within the step's memory bound.  The row and target tensors are
+        built here, after the layers (device-side fills and slices of the staged ids: no host-to-device copy, no sync)."""
+        K, n, dev = st.num_rows, st.top_n, input_embds.device
+        ids = st.input_ids
+        rows = torch.cat([torch.arange(s, s + c - 1 + (nx is not None), dtype=torch.int32, device=dev) for s, c, nx in st.pieces])
+        targets = torch.cat([t for s, c, nx in st.pieces
+                             for t in (ids[s + 1:s + c],) + (() if nx is None else (ids.new_full((1,), nx),))])
+        assert rows.shape[0] == K and targets.shape[0] == K
+        res = (torch.empty((K,), dtype=torch.float32, device=dev), torch.empty((K,), dtype=torch.int32, device=dev),
+               torch.empty((K, n), dtype=torch.int32, device=dev), torch.empty((K, n), dtype=torch.float32, device=dev))
+        kept = []
+        for b0 in range(0, K, st.block_rows):
+            b1 = min(K, b0 + st.block_rows)
+            x = input_embds.index_select(0, rows[b0:b1])
+            if not already_normed:
+                rmsnorm_inplace(x, self.weights.final_norm, self.model_config.rms_norm_eps)
+            logits = linear(x, self.weights.lm_head)
+            del x
+            if self.sharded:
+                logits = self._gather_logits(logits)
+            prompt_logprobs(logits, targets[b0:b1], n, out=tuple(t[b0:b1] for t in res))
+            if self.keep_logits:
+                kept.append(logits.clone())
+            del logits
+        if self.keep_logits:                                   # parity tests only
+            self.last_prompt_logits = torch.cat(kept)
+        return res
+
+    def _last_rows(self, input_embds: torch.Tensor, infer_state: LlamaInferState, already_normed: bool):
         idx = infer_state.last_token_indices
         if idx is None:
             idx = torch.cat((

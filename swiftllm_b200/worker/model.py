@@ -3,7 +3,8 @@
 
     LlamaModel(engine_config) -> load_weights() -> profile_num_blocks() -> init_kvcache_and_swap(num_blocks)
     forward(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False) -> list[int]
-    forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities)
+    forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities,
+                                                            and of prompt tokens with SamplingParams.prompt_logprobs)
     forward_speculative(input_ids_list, seq_ids_list, prefix_lens_list, sampling_params_list=None) -> list[list[int]]
                                                             (addition: verify up to 7 drafts per sequence in one step)
     fork_seqs(src_seq_ids_list, dst_seq_ids_list, lens_list)  (addition: share a cached prefix with another sequence)
@@ -31,13 +32,14 @@ import torch.distributed as dist
 from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
-from swiftllm_b200.sampling_params import TokenLogprobs, has_penalties, logprobs_top_n, sampling_words
+from swiftllm_b200.sampling_params import (PromptLogprobs, SamplingParams, TokenLogprobs, has_penalties, logprobs_top_n, prompt_logprobs_top_n,
+                                           sampling_words)
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.kernels.block_mgmt import copy_block_tails
 from swiftllm_b200.worker.weight import load_weights
 
-from .infer_state import LlamaInferState, SamplingState
+from .infer_state import LlamaInferState, PromptLogprobsState, SamplingState
 from .layers.post_layer import LlamaPostLayer
 from .layers.pre_layer import LlamaPreLayer
 from .layers.transformer_layer import LlamaTransformerLayer
@@ -339,26 +341,97 @@ class LlamaModel:
     @torch.inference_mode()
     def forward_with_logprobs(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
                               ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
-                              sampling_params_list: Optional[list] = None) -> list:
-        """forward() that also returns log-probabilities: one swiftllm_b200.TokenLogprobs(token, logprob, top) per batch entry.
-        Entry i gets them when sampling_params_list[i].logprobs is not None: the log-probability of its token and, for
+                              sampling_params_list: Optional[list] = None, prompt_next_ids_list: Optional[list] = None) -> list:
+        """forward() that also returns log-probabilities: one swiftllm_b200.TokenLogprobs(token, logprob, top, prompt) per batch
+        entry.  Entry i gets them when sampling_params_list[i].logprobs is not None: the log-probability of its token and, for
         logprobs = N > 0, the N most likely tokens as (id, logprob), most likely first, ties broken by the smaller id.  They are
         log_softmax of the raw logits the token was chosen from (csrc/logprobs.cu), not of the temperature-scaled or filtered
-        distribution.  The tokens are the ones forward() returns for the same arguments."""
+        distribution.  The tokens are the ones forward() returns for the same arguments.
+
+        A prefill entry with sampling_params_list[i].prompt_logprobs set also gets `prompt`, a swiftllm_b200.PromptLogprobs: each
+        of its rows scores the prompt token after it (csrc/prompt_logprobs.cu, the same values as above).  The last row of the
+        entry scores prompt_next_ids_list[i] when that is given (one entry per prefill entry, None or the id of the prompt token
+        after this chunk); so chunks of a prompt, each given the next chunk's first token, together score positions 1 .. P - 1.
+        The step's tokens and KV-cache writes are those of forward().  A prompt_next_ids_list of the wrong length, or an id of an
+        asking entry outside [0, vocab_size), raises ValueError before anything is enqueued."""
+        plan = self._prompt_plan(input_ids_list, decoding_seq_lens_list, prefill_prefix_lens_list, sampling_params_list,
+                                 prompt_next_ids_list)
         out = self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-                         sampling_params_list, with_logprobs=True)
-        if isinstance(out, torch.Tensor):                   # no entry asked: forward()'s step
-            return [TokenLogprobs(t) for t in out.tolist()]
-        tokens, token_lp, top_ids, top_lp = (t.tolist() for t in out)
-        res = []
-        for i, t in enumerate(tokens):
-            n = sampling_params_list[i].logprobs
-            if n is None:
-                res.append(TokenLogprobs(t))
-            else:
-                n = min(int(n), self.model_config.vocab_size)
-                res.append(TokenLogprobs(t, token_lp[i], list(zip(top_ids[i][:n], top_lp[i][:n]))))
+                         sampling_params_list, with_logprobs=True, prompt_plan=plan if plan and plan["num_rows"] else None)
+        prompt_out = None
+        if plan and plan["num_rows"]:
+            out, prompt_out = out
+        if isinstance(out, torch.Tensor):                   # no entry asked for the returned token's log-probabilities
+            res = [TokenLogprobs(t) for t in out.tolist()]
+        else:
+            tokens, token_lp, top_ids, top_lp = (t.tolist() for t in out)
+            res = []
+            for i, t in enumerate(tokens):
+                n = sampling_params_list[i].logprobs
+                if n is None:
+                    res.append(TokenLogprobs(t))
+                else:
+                    n = min(int(n), self.model_config.vocab_size)
+                    res.append(TokenLogprobs(t, token_lp[i], list(zip(top_ids[i][:n], top_lp[i][:n]))))
+        if plan:
+            lp, rank, ids, tlp = (t.cpu().numpy() for t in prompt_out) if prompt_out is not None else (None,) * 4
+            for i, first, off, k, n in plan["entries"]:
+                tgt = np.asarray(plan["targets"][off:off + k], dtype=np.int64)
+                if k == 0:
+                    pl = PromptLogprobs(first, tgt, np.zeros((0,), np.float32), np.zeros((0,), np.int32),
+                                        np.zeros((0, n), np.int32), np.zeros((0, n), np.float32))
+                else:
+                    pl = PromptLogprobs(first, tgt, lp[off:off + k].copy(), rank[off:off + k].copy(),
+                                        ids[off:off + k, :n].copy(), tlp[off:off + k, :n].copy())
+                res[i] = res[i]._replace(prompt=pl)
         return res
+
+    def _prompt_plan(self, input_ids_list, decoding_seq_lens_list, prefill_prefix_lens_list, sampling_params_list,
+                     prompt_next_ids_list):
+        """Host plan of the prompt rows of forward_with_logprobs, None when no prefill entry asks: entries [(batch index, first
+        position, offset into the rows, rows k, N)], pieces [(first row of the entry in the activation matrix, its token
+        count n, next id or None)] of the entries with rows to score, the number of rows, the targets and the per-launch N.
+        Validates prompt_next_ids_list (ValueError)."""
+        P = len(input_ids_list) - len(decoding_seq_lens_list)
+        if prompt_next_ids_list is not None and len(prompt_next_ids_list) != P:
+            raise ValueError(f"prompt_next_ids_list has {len(prompt_next_ids_list)} entries for {P} prefill entries")
+        if sampling_params_list is None or len(sampling_params_list) != len(input_ids_list):
+            return None                                     # sampling_words raises for a list of the wrong length
+        for sp in sampling_params_list[:P]:
+            if not isinstance(sp, SamplingParams):
+                return None                                 # sampling_words raises
+            sp.validate()
+        top_n = prompt_logprobs_top_n(sampling_params_list[:P])
+        if top_n is None:
+            return None
+        V = self.model_config.vocab_size
+        prefix = [int(x) for x in prefill_prefix_lens_list] if prefill_prefix_lens_list is not None else [0] * P
+        entries, pieces, targets = [], [], []
+        start = 0
+        for i in range(P):
+            ids, n_i = input_ids_list[i], len(input_ids_list[i])
+            n = sampling_params_list[i].prompt_logprobs
+            if n is not None:
+                nxt = None if prompt_next_ids_list is None else prompt_next_ids_list[i]
+                if nxt is not None and (isinstance(nxt, bool) or not isinstance(nxt, (int, np.integer)) or not 0 <= nxt < V):
+                    raise ValueError(f"prompt_next_ids_list[{i}] must be None or a token id in [0, {V}), got {nxt!r}")
+                k = max(n_i - 1, 0) + (nxt is not None and n_i > 0)
+                entries.append((i, prefix[i] + 1, len(targets), k, min(int(n), V)))
+                targets += [int(x) for x in ids[1:]]
+                if nxt is not None and n_i > 0:
+                    targets.append(int(nxt))
+                if k > 0:
+                    pieces.append((start, n_i, None if nxt is None else int(nxt)))
+            start += n_i
+        return dict(entries=entries, pieces=pieces, num_rows=len(targets), targets=targets, top_n=top_n)
+
+    def _prompt_block_rows(self) -> int:
+        """Rows per prompt-logprobs block: the block's logits (and with a sharded lm_head the shard and the gathered copy) stay
+        within the [max_tokens_in_batch, 2 * ffn_inter_dim / tp] up_gate output of the forward profile_num_blocks measures."""
+        mc = self.model_config
+        V = mc.vocab_size
+        per_row = 2 * V + V // self.tp_size if self.post_layer.sharded else V
+        return max(1, self.engine_config.max_tokens_in_batch * 2 * (mc.ffn_inter_dim // self.tp_size) // per_row)
 
     MAX_SPECULATIVE_ROWS = 8
 
@@ -447,9 +520,12 @@ class LlamaModel:
         return out
 
     def _step(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-              sampling_params_list, with_logprobs: bool):
+              sampling_params_list, with_logprobs: bool, prompt_plan: Optional[dict] = None):
         """One step: the token tensor, or with log-probabilities asked for by some entry (with_logprobs and a
-        SamplingParams.logprobs set) the tuple (tokens, token logprobs, top ids, top logprobs) on the device."""
+        SamplingParams.logprobs set) the tuple (tokens, token logprobs, top ids, top logprobs) on the device.  With a
+        `prompt_plan` (forward_with_logprobs._prompt_plan, some rows to score): (that, (prompt logprobs, ranks, top ids, top
+        logprobs)).  The step stages exactly what it stages without one: the post layer builds the rows and targets on the device
+        after the layers, so nothing of the prompt part is allocated while the forward's activations are."""
         mc = self.model_config
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
@@ -494,6 +570,9 @@ class LlamaModel:
             *([samp[0]] if samp else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens, prefill_starts, positions,
             last_idx, prefix_lens if chunked else [])
         ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = views[-8:]
+        pp = prompt_plan
+        prompt_state = None if pp is None else PromptLogprobsState(
+            pieces=pp["pieces"], num_rows=pp["num_rows"], input_ids=ids, top_n=pp["top_n"], block_rows=self._prompt_block_rows())
         sampling = SamplingState.from_staged(views[0], seq_lengths, samp[1]) if samp else None
         if penalized:
             sampling = dataclasses.replace(sampling, sampled=sampled, input_ids=ids,
@@ -523,7 +602,7 @@ class LlamaModel:
             paged_attn_seq_block_size=0, last_token_indices=last,
             prefill_prefix_lens=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0,
-            sampling=sampling, logprobs=top_n,
+            sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state,
         )
         return self._forward(ids, infer_state)
 
