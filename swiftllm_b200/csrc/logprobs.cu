@@ -10,12 +10,14 @@
 //              keys); a -inf logit of an otherwise finite row gives -inf.
 // The result is a pure function of the row: it does not depend on the batch, the cluster size or the launch mode.
 //
-// Layout: one thread-block cluster of C CTAs per row, C and the slices as in sampling.cu.  Each CTA stages its slice as keys in
-// shared memory (HBM read once); the passes are the max (with the NaN / +inf flag and per-warp maxima), Z together with the
-// high-byte count histogram, the low-byte histogram (an exact radix select of tau, the N-th largest key; only keys >= the N-th
-// largest warp maximum, a lower bound of tau, are counted, which keeps the shared-memory atomics few), and one in-order pass that takes every
-// key > tau and the lowest-id ties at tau.  CTAs own increasing id ranges, so per-CTA tie counts in rank order tell each CTA
-// how many of its ties to take.  Rank 0 gathers the <= 20 survivors over DSMEM and one warp sorts them.
+// Layout: one thread-block cluster of C CTAs per row; C, the slices, the launch, the staging and the two-byte select are
+// vocab_select.cuh's, as in sampling.cu, and Z and lse go through the mass_of / lse_of that prompt_logprobs.cu also uses.
+// Each CTA stages its slice as keys in shared memory (HBM read once); the passes are the max (with the NaN / +inf flag and
+// per-warp maxima), Z together with the high-byte count histogram, the low-byte histogram (an exact radix select of tau, the
+// N-th largest key; only keys >= the N-th largest warp maximum, a lower bound of tau, are counted, which keeps the
+// shared-memory atomics few), and one in-order pass that takes every key > tau and the lowest-id ties at tau.  CTAs own
+// increasing id ranges, so per-CTA tie counts in rank order tell each CTA how many of its ties to take.  Rank 0 gathers the
+// <= 20 survivors over DSMEM and one warp sorts them.
 // Algorithmic bytes: rows * V * 2 (logits) + rows * (12 + 8 * top_n).
 //
 // No fast-math here: expf / logf must be the accurate ones the restatement's tolerance is derived for.
@@ -56,33 +58,10 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
     if (threadIdx.x == 0) cand_n = 0;
     unsigned long long best = 0;
     bool bad = false;
-    auto see = [&](uint32_t k) {
+    stage_keys(reinterpret_cast<const uint16_t*>(src), n, keys, [&](uint32_t k, int) {
         best = k > best ? k : best;
         bad |= k >= InfKeys<T>::pos || k < InfKeys<T>::neg;
-    };
-    const uint16_t* s16 = reinterpret_cast<const uint16_t*>(src);
-    int vec_end = 0;
-    if ((reinterpret_cast<uintptr_t>(src) & 15) == 0) {
-        vec_end = n & ~7;
-        for (int i = 8 * threadIdx.x; i < vec_end; i += 8 * blockDim.x) {
-            uint4 u;
-            asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-                         : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(s16 + i));
-            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-            uint32_t k[8];
-#pragma unroll
-            for (int j = 0; j < 4; j++) { k[2 * j] = key_of((uint16_t)(w[j] & 0xffffu)); k[2 * j + 1] = key_of((uint16_t)(w[j] >> 16)); }
-#pragma unroll
-            for (int j = 0; j < 8; j++) see(k[j]);
-            *reinterpret_cast<uint4*>(keys + i) = make_uint4(k[0] | (k[1] << 16), k[2] | (k[3] << 16), k[4] | (k[5] << 16),
-                                                              k[6] | (k[7] << 16));
-        }
-    }
-    for (int i = vec_end + threadIdx.x; i < n; i += blockDim.x) {
-        const uint32_t k = key_of(s16[i]);
-        keys[i] = (uint16_t)k;
-        see(k);
-    }
+    });
     const uint32_t wmax = __reduce_max_sync(0xffffffffu, (uint32_t)best);
     if (lane == 0) warp_max[warp] = wmax;
     best = block_max_u64(best, scratch);
@@ -105,13 +84,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
         const unsigned wpc = blockDim.x >> 5;
         if (threadIdx.x < W) all_warp_max[threadIdx.x] = cluster.map_shared_rank(warp_max, threadIdx.x / wpc)[threadIdx.x % wpc];
         __syncthreads();
-        if (threadIdx.x < W) {
-            const uint32_t v = all_warp_max[threadIdx.x];
-            int gt = 0, ge = 0;
-            for (int j = 0; j < W; j++) { gt += all_warp_max[j] > v; ge += all_warp_max[j] >= v; }
-            if (gt < N && N <= ge) floor_key = v;                     // threads that write hold the same value
-        }
-        __syncthreads();
+        nth_largest(all_warp_max, W, N, &floor_key);
     }
     const uint32_t lowest = N > 0 ? floor_key : 0u;
 
@@ -120,7 +93,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
     for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
         const int i = i0 + lane;
         const uint32_t key = i < n ? keys[i] : 0u;
-        if (!bad && i < n) z += __float2ull_rn(__fmul_rn(expf(__fsub_rn(value_of<T>(key), m)), kMassScale));
+        if (!bad && i < n) z += mass_of<T>(key, m);
         if (N > 0) warp_hist_add(h_hi, i < n && key >= lowest, key >> 8, 1ull);
     }
     z = block_sum_u64(z, scratch);
@@ -130,16 +103,11 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
         // ---- tau = the N-th largest key (radix select over the two bytes of the keys >= floor), `above` = keys > tau in the row
         merge_hist(cluster, h_hi, merged);
         select_bin(merged, 0, (double)N, &sel_bin, &sel_above);
-        const uint32_t hi = (uint32_t)sel_bin;
-        for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
-            const int i = i0 + lane;
-            const uint32_t key = i < n ? keys[i] : 0u;
-            warp_hist_add(h_lo, i < n && key >= lowest && (key >> 8) == hi, key & 255, 1ull);
-        }
-        merge_hist(cluster, h_lo, merged);
-        select_bin(merged, sel_above, (double)N, &sel_bin, &sel_above);
-        const uint32_t lo = (uint32_t)sel_bin, tau = (hi << 8) | lo;
-        const int need_ties = N - (int)sel_above;                     // >= 1
+        const Selected sel = select_low_byte(cluster, keys, n, (uint32_t)sel_bin, sel_above, merged, h_lo, (double)N,
+                                             [&](uint32_t key) { return key >= lowest; },
+                                             [](uint32_t, bool) { return 1ull; }, &sel_bin, &sel_above);
+        const uint32_t tau = sel.tau, lo = tau & 255;
+        const int need_ties = N - (int)sel.above;                     // >= 1
 
         // ---- this CTA's share of the ties: the lowest ids first, and CTAs own increasing id ranges
         int prior = 0;
@@ -175,7 +143,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
     if (rank == 0 && warp == 0) {
         unsigned long long Z = 0;
         for (unsigned r = 0; r < C; r++) Z += *cluster.map_shared_rank(&cta_z, r);
-        const float lse = bad ? NAN : __fadd_rn(m, logf(__fmul_rn(__ull2float_rn(Z), 1.0f / kMassScale)));
+        const float lse = bad ? NAN : lse_of(m, Z);
         if (N > 0) {
             uint32_t k = 0;
             int32_t id = INT32_MAX;
@@ -199,10 +167,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
                 out_top_logprobs[row * top_n + place] = __fsub_rn(value_of<T>(k), lse);
             }
         }
-        for (int j = N + lane; j < top_n; j += 32) {
-            out_top_ids[row * top_n + j] = -1;
-            out_top_logprobs[row * top_n + j] = NAN;
-        }
+        fill_top_tail(out_top_ids + row * top_n, out_top_logprobs + row * top_n, N, top_n, lane, 32);
         if (lane == 0) {
             const int64_t tok = token_ids[row];
             float lp = NAN;
@@ -212,35 +177,6 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const T* __restrict_
         }
     }
     cluster.sync();                                                   // peers' shared memory stays valid until rank 0 has read it
-}
-
-template <typename T>
-int launch(const void* logits, int64_t rows, int V, int64_t row_stride, const int64_t* token_ids, int top_n,
-           float* out_token_logprob, int32_t* out_top_ids, float* out_top_logprobs, cudaStream_t stream) {
-    const int C = cluster_size(rows, V);
-    const int slice = ((V + C - 1) / C + 7) & ~7;
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(logprobs_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSliceBytes);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(rows * C));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = (size_t)slice * sizeof(uint16_t);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, logprobs_kernel<T>, (const T*)logits, row_stride, V, slice, token_ids, top_n,
-                                       out_token_logprob, out_top_ids, out_top_logprobs);
-    if (e != cudaSuccess) {
-        set_error("token_logprobs: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return check_launch("token_logprobs");
 }
 
 }  // namespace
@@ -253,7 +189,7 @@ extern "C" int sllm_token_logprobs(const void* logits, int64_t num_rows, int voc
     SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "token_logprobs: unsupported dtype tag %d", (int)dtype);
     SLLM_REQUIRE(num_rows >= 0 && num_rows <= (1 << 20), "token_logprobs: num_rows %lld out of range", (long long)num_rows);
     SLLM_REQUIRE(vocab_size > 0, "token_logprobs: vocab_size must be positive, got %d", vocab_size);
-    SLLM_REQUIRE(((int64_t)(vocab_size + kMaxCluster - 1) / kMaxCluster + 7) / 8 * 8 * 2 <= kMaxSliceBytes,
+    SLLM_REQUIRE(slice_fits(vocab_size, kMaxCluster, kKeyBytes, kKeyAlign),
                  "token_logprobs: vocab_size %d does not fit the shared memory of a %d-CTA cluster", vocab_size, kMaxCluster);
     SLLM_REQUIRE(top_n >= 0 && top_n <= kMaxTopN, "token_logprobs: top_n %d outside [0, %d]", top_n, kMaxTopN);
     SLLM_REQUIRE(logits_row_stride >= vocab_size, "token_logprobs: logits_row_stride %lld < vocab_size %d",
@@ -261,6 +197,9 @@ extern "C" int sllm_token_logprobs(const void* logits, int64_t num_rows, int voc
     if (num_rows == 0) return 0;
     SLLM_REQUIRE(logits && token_ids && out_token_logprob && (top_n == 0 || (out_top_ids && out_top_logprobs)),
                  "token_logprobs: null pointer");
-    SLLM_DISPATCH_DTYPE(dtype, return launch<T>(logits, num_rows, vocab_size, logits_row_stride, token_ids, top_n,
-                                                out_token_logprob, out_top_ids, out_top_logprobs, (cudaStream_t)stream));
+    const ClusterGeometry g = cluster_geometry(num_rows, vocab_size, kKeyBytes, kKeyAlign);
+    SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<logprobs_kernel<T>>(
+                                   num_rows, g.C, (size_t)g.slice * kKeyBytes, (cudaStream_t)stream, "token_logprobs",
+                                   (const T*)logits, logits_row_stride, vocab_size, g.slice, token_ids, top_n, out_token_logprob,
+                                   out_top_ids, out_top_logprobs));
 }

@@ -11,8 +11,9 @@
 // is skipped, never dereferenced.  Rows with r == 1, f == 0, p == 0 are skipped entirely (nothing read, recorded or modified).
 // After counting, the row's new tokens are written to positions [pos - n_new, pos) of its pages - disjoint from what is read.
 //
-// Layout: one thread-block cluster of C CTAs per penalised row.  The cluster keeps a u32 slot per vocabulary id of the launch's
-// shard in distributed shared memory, CTA k owning ids [k * slice, (k + 1) * slice): bit 31 = seen in the prompt, the low bits
+// Layout: one thread-block cluster of C CTAs per penalised row, with the cluster geometry (4 bytes per entry) and launch of
+// vocab_select.cuh.  The cluster keeps a u32 slot per vocabulary id of the launch's shard in distributed shared memory, CTA k
+// owning ids [k * slice, (k + 1) * slice): bit 31 = seen in the prompt, the low bits
 // count output tokens (exact up to 2^31 - 1).  Every CTA counts a strided share of the history into whichever CTA owns each id;
 // lanes of a warp holding the same (id, kind) are merged first (__match_any_sync), so one id repeated thousands of times costs one
 // DSMEM atomic per warp, not one per occurrence.  After a cluster barrier each CTA rewrites the entries of its slice whose slot
@@ -27,20 +28,7 @@ constexpr uint32_t kOutputBit = 0x80000000u;       // token page word: id | kOut
 constexpr uint32_t kSeenInPrompt = 0x80000000u;    // cluster slot: set when the id occurs among the prompt tokens
 constexpr uint32_t kAbsentId = 0x7fffffffu;        // recorded for a negative input id: >= vocab_offset + vocab_size always
 
-// Cluster size for 4-byte slots: the smallest that fits a slice in shared memory, raised towards rows * C >= the SM count.
-int penalty_cluster_size(int64_t rows, int V) {
-    int c = 1;
-    while (c < kMaxCluster && (((int64_t)V + c - 1) / c + 3) / 4 * 4 * 4 > kMaxSliceBytes) c *= 2;
-    while (c < kMaxCluster && rows * c * 2 <= 132) c *= 2;
-    return c;
-}
-
-template <typename T> __device__ __forceinline__ float to_f32(T x);
-template <> __device__ __forceinline__ float to_f32<__half>(__half x) { return __half2float(x); }
-template <> __device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
-template <typename T> __device__ __forceinline__ T from_f32(float x);
-template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
-template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+constexpr int kSlotBytes = 4, kSlotAlign = 4;     // cluster slots: uint32, slices zeroed as whole uint4 vectors
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads) penalty_kernel(
@@ -113,11 +101,11 @@ __global__ void __launch_bounds__(kThreads) penalty_kernel(
         const uint32_t c = slots[j];
         if (c == 0) continue;
         const uint32_t c_out = c & ~kSeenInPrompt;
-        float l = to_f32<T>(dst[j]);
+        float l = Traits<T>::to_f(dst[j]);
         l = l > 0.f ? __fdiv_rn(l, r) : __fmul_rn(l, r);
         float t = __fmul_rn(f, __uint2float_rn(c_out));
         if (c_out > 0) t = __fadd_rn(t, p);
-        dst[j] = from_f32<T>(__fsub_rn(l, t));
+        dst[j] = Traits<T>::from_f(__fsub_rn(l, t));
     }
 
     // ---- record this step's tokens at positions [P - n_new, P)
@@ -126,39 +114,6 @@ __global__ void __launch_bounds__(kThreads) penalty_kernel(
         if (s >= 0) token_cache[s] = (int32_t)new_word(j);
     }
     // no DSMEM access after the last barrier: peers may leave
-}
-
-template <typename T>
-int launch(void* logits, int64_t rows, int V, int64_t row_stride, int64_t vocab_offset, const float* rep, const float* freq,
-           const float* pres, const int32_t* seq_ids, const int32_t* pos, const int32_t* input_ids,
-           const int32_t* last_token_indices, const int32_t* prefill_seq_lens, int num_prefill_rows,
-           const int32_t* block_table, int block_table_stride, int block_size, int32_t* token_cache, int64_t num_blocks,
-           cudaStream_t stream) {
-    const int C = penalty_cluster_size(rows, V);
-    const int slice = ((V + C - 1) / C + 3) & ~3;
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(penalty_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSliceBytes);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(rows * C));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = (size_t)slice * sizeof(uint32_t);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, penalty_kernel<T>, (T*)logits, row_stride, V, vocab_offset, slice, rep, freq, pres,
-                                       seq_ids, pos, input_ids, last_token_indices, prefill_seq_lens, num_prefill_rows,
-                                       block_table, block_table_stride, block_size, token_cache, num_blocks);
-    if (e != cudaSuccess) {
-        set_error("apply_penalties: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return check_launch("apply_penalties");
 }
 
 }  // namespace
@@ -175,7 +130,7 @@ extern "C" int sllm_apply_penalties(void* logits, int64_t num_rows, int vocab_si
     SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "apply_penalties: unsupported dtype tag %d", (int)dtype);
     SLLM_REQUIRE(num_rows >= 0 && num_rows <= (1 << 20), "apply_penalties: num_rows %lld out of range", (long long)num_rows);
     SLLM_REQUIRE(vocab_size > 0, "apply_penalties: vocab_size must be positive, got %d", vocab_size);
-    SLLM_REQUIRE(((((int64_t)vocab_size + kMaxCluster - 1) / kMaxCluster + 3) & ~3ll) * 4 <= kMaxSliceBytes,
+    SLLM_REQUIRE(slice_fits(vocab_size, kMaxCluster, kSlotBytes, kSlotAlign),
                  "apply_penalties: vocab_size %d does not fit the shared memory of a %d-CTA cluster", vocab_size, kMaxCluster);
     SLLM_REQUIRE(vocab_offset >= 0 && vocab_offset + vocab_size <= (int64_t)INT32_MAX,
                  "apply_penalties: global vocabulary indices must stay below 2^31 (vocab_offset %lld)", (long long)vocab_offset);
@@ -191,9 +146,11 @@ extern "C" int sllm_apply_penalties(void* logits, int64_t num_rows, int vocab_si
     SLLM_REQUIRE(logits && repetition_penalty && frequency_penalty && presence_penalty && seq_ids && pos && input_ids &&
                  last_token_indices && block_table && token_cache && (num_prefill_rows == 0 || prefill_seq_lens),
                  "apply_penalties: null pointer");
-    SLLM_DISPATCH_DTYPE(dtype, return launch<T>(logits, num_rows, vocab_size, logits_row_stride, vocab_offset,
-                                                repetition_penalty, frequency_penalty, presence_penalty, seq_ids, pos,
-                                                input_ids, last_token_indices, prefill_seq_lens, num_prefill_rows, block_table,
-                                                block_table_stride, block_size, token_cache, num_blocks,
-                                                (cudaStream_t)stream));
+    const ClusterGeometry g = cluster_geometry(num_rows, vocab_size, kSlotBytes, kSlotAlign);
+    SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<penalty_kernel<T>>(
+                                   num_rows, g.C, (size_t)g.slice * kSlotBytes, (cudaStream_t)stream, "apply_penalties",
+                                   (T*)logits, logits_row_stride, vocab_size, vocab_offset, g.slice, repetition_penalty,
+                                   frequency_penalty, presence_penalty, seq_ids, pos, input_ids, last_token_indices,
+                                   prefill_seq_lens, num_prefill_rows, block_table, block_table_stride, block_size, token_cache,
+                                   num_blocks));
 }

@@ -1,9 +1,10 @@
 // Prompt log-probabilities: for each of many [rows, V] logits rows (every row of a prefill), the log-probability of a given
 // target token, its rank and the top-N entries of log_softmax(l).  The values are those of sllm_token_logprobs
 // (csrc/logprobs.cu) bit for bit: m (the largest key), Z = sum over v of round(expf(l_v - m) * 2^40) as 64-bit integers,
-// lse = m + logf(Z * 2^-40) and l - lse, with the same intrinsics.  Z is an exact integer, so how the row is partitioned among
-// threads does not change it.  rank = 1 + the number of ids whose key (vocab_select.cuh: order-preserving, -0 == +0) is strictly
-// greater than the target's; a target outside [0, V) gives NaN and rank -1.  Top-N, NaN / +inf rows: as csrc/logprobs.cu.
+// lse = m + logf(Z * 2^-40) and l - lse, through the same mass_of / lse_of (vocab_select.cuh).  Z is an exact integer, so how
+// the row is partitioned among threads does not change it.  rank = 1 + the number of ids whose key (vocab_select.cuh:
+// order-preserving, -0 == +0) is strictly greater than the target's; a target outside [0, V) gives NaN and rank -1.  Top-N,
+// NaN / +inf rows: as csrc/logprobs.cu.
 //
 // Layout: one CTA of 512 threads per row, no clusters; two or more CTAs per SM, so one row's arithmetic overlaps another's loads.
 //   pass 1  streams the row from HBM: the largest key, the NaN / +inf flag, the count of keys above the target's key and the
@@ -14,6 +15,7 @@
 //   select  each candidate's place among the others by (key desc, id asc); places below N are the top-N.  A row with more than
 //           kMaxCand candidates (many ties near its top) takes N block-wide max rounds over its (key, id) pairs instead: exact,
 //           slower, and only reached by degenerate rows.
+// The row load, keys8 / pack8, pair_of, the floor (nth_largest) and the block reductions are vocab_select.cuh's.
 // Algorithmic bytes: rows * V * 2 (logits) + rows * (12 + 8 * top_n).
 //
 // No fast-math here: expf / logf must be the accurate ones csrc/logprobs.cu uses.
@@ -30,31 +32,6 @@ constexpr int kMaxCand = 1024;
 constexpr int kStageKeys = 48 * 1024;                    // 96 KB of staged keys per CTA: two CTAs of the largest vocabularies per SM
 constexpr int kMaxPromptRows = 1 << 24;
 constexpr int kMaxPromptVocab = 1 << 24;                 // Z <= V * 2^40 stays below 2^64
-
-// 16 logits bytes that bypass L1; `last_use`: read for the last time, so L2 evicts them first (the part of the row pass 2 reads
-// again keeps the normal priority)
-__device__ __forceinline__ uint4 ld_row_vec(const uint4* p, bool last_use) {
-    uint4 u;
-    if (last_use)
-        asm volatile("{\n\t.reg .b64 pol;\n\tcreatepolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
-                     "ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], pol;\n\t}"
-                     : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(p));
-    else
-        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-                     : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(p));
-    return u;
-}
-
-__device__ __forceinline__ void keys8(const uint4& u, uint32_t (&k)[8]) {
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; j++) { k[2 * j] = key_of((uint16_t)(w[j] & 0xffffu)); k[2 * j + 1] = key_of((uint16_t)(w[j] >> 16)); }
-}
-
-// (key desc, id asc) as one unsigned order: larger is better, and no two ids share a value
-__device__ __forceinline__ unsigned long long pair_of(uint32_t key, int id) {
-    return ((unsigned long long)key << 32) | (0xffffffffu - (uint32_t)id);
-}
 
 template <typename T>
 __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
@@ -93,10 +70,10 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
     };
     for (int j = tid; j < nvec; j += kRowThreads) {
         uint32_t k[8];
-        keys8(ld_row_vec(vsrc + j, j < nstage), k);
+        keys8(ld_row16(vsrc + j, j < nstage), k);
 #pragma unroll
         for (int e = 0; e < 8; e++) see(k[e]);
-        if (j < nstage) staged[j] = make_uint4(k[0] | (k[1] << 16), k[2] | (k[3] << 16), k[4] | (k[5] << 16), k[6] | (k[7] << 16));
+        if (j < nstage) staged[j] = pack8(k);
     }
     for (int t = tid; t < nscalar; t += kRowThreads) see(key_of(s16[scalar_id(t)]));
     uint32_t g = best;
@@ -118,21 +95,13 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
     bad |= m == -INFINITY;                               // every logit -inf: no distribution (NaN, as log_softmax)
 
     // ---- the top-N floor: the N-th largest group maximum (a group without keys reports 0, which can only lower it)
-    if (N > 0) {
-        if (tid < kGroups) {
-            const uint32_t v = group_max[tid];
-            int gt = 0, ge = 0;
-            for (int j = 0; j < kGroups; j++) { gt += group_max[j] > v; ge += group_max[j] >= v; }
-            if (gt < N && N <= ge) floor_key = v;        // threads that write hold the same value
-        }
-        __syncthreads();
-    }
+    if (N > 0) nth_largest(group_max, kGroups, N, &floor_key);
     const uint32_t lowest = N > 0 ? floor_key : 0u;
 
     // ---- pass 2: Z (exact fixed point) and the candidates >= floor; the re-read part first, while it is in L2
     unsigned long long z = 0;
     auto take = [&](uint32_t k, int id) {
-        if (!bad) z += __float2ull_rn(__fmul_rn(expf(__fsub_rn(value_of<T>(k), m)), kMassScale));
+        if (!bad) z += mass_of<T>(k, m);
         if (N > 0 && k >= lowest) {
             const int s = atomicAdd(&cand_n, 1);
             if (s < kMaxCand) cand[s] = pair_of(k, id);
@@ -140,7 +109,7 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
     };
     for (int j = nstage + tid; j < nvec; j += kRowThreads) {
         uint32_t k[8];
-        keys8(ld_row_vec(vsrc + j, true), k);
+        keys8(ld_row16(vsrc + j, true), k);
 #pragma unroll
         for (int e = 0; e < 8; e++) take(k[e], head + 8 * j + e);
     }
@@ -152,7 +121,7 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
         for (int e = 0; e < 8; e++) take((w[e >> 1] >> (16 * (e & 1))) & 0xffffu, head + 8 * j + e);
     }
     const unsigned long long Z = block_sum_u64(z, scratch);     // ends with every thread past a __syncthreads: cand_n is final
-    const float lse = bad ? NAN : __fadd_rn(m, logf(__fmul_rn(__ull2float_rn(Z), 1.0f / kMassScale)));
+    const float lse = bad ? NAN : lse_of(m, Z);
 
     // ---- select the top-N: (key desc, id asc)
     const int64_t o = row * top_n;
@@ -183,10 +152,7 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
             prev = b;
         }
     }
-    for (int j = N + tid; j < top_n; j += kRowThreads) {
-        out_top_ids[o + j] = -1;
-        out_top_logprobs[o + j] = NAN;
-    }
+    fill_top_tail(out_top_ids + o, out_top_logprobs + o, N, top_n, tid, kRowThreads);
     if (tid == 0) {
         out_logprob[row] = tok_ok ? __fsub_rn(value_of<T>(tok_key), lse) : NAN;
         out_rank[row] = tok_ok ? (int32_t)(1 + total_above) : -1;

@@ -14,7 +14,9 @@
 //
 // Layout: one thread-block cluster of C CTAs per row (C chosen on the host so that rows * C covers the GPU at small batch).  Each
 // CTA stages its contiguous slice of the row in shared memory as keys (HBM read once), every pass runs from there, and the
-// per-CTA histograms / maxima / best (score, index) pairs are merged through distributed shared memory.
+// per-CTA histograms / maxima / best (score, index) pairs are merged through distributed shared memory.  The staging, the
+// two-byte select of both thresholds, the cluster geometry and the launch are those of vocab_select.cuh; the top-p mass
+// (divided by T) is this kernel's own.
 // Algorithmic bytes: rows * V * 2 (logits) + rows * 32 (parameters and result).
 //
 // No fast-math here: logf / expf / division must be the accurate ones the restatement reproduces.
@@ -70,33 +72,10 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     // ---- stage the slice as keys; local (max key, smallest index)
     for (int i = threadIdx.x; i < 256; i += blockDim.x) h_cnt_hi[i] = h_cnt_lo[i] = h_mass_hi[i] = h_mass_lo[i] = 0;
     unsigned long long best = 0;
-    const uint16_t* s16 = reinterpret_cast<const uint16_t*>(src);
-    int vec_end = 0;
-    if ((reinterpret_cast<uintptr_t>(src) & 15) == 0) {
-        vec_end = n & ~7;
-        for (int i = 8 * threadIdx.x; i < vec_end; i += 8 * blockDim.x) {
-            uint4 u;
-            asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-                         : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(s16 + i));
-            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-            uint32_t k[8];
-#pragma unroll
-            for (int j = 0; j < 4; j++) { k[2 * j] = key_of((uint16_t)(w[j] & 0xffffu)); k[2 * j + 1] = key_of((uint16_t)(w[j] >> 16)); }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const unsigned long long c = ((unsigned long long)k[j] << 32) | (0xffffffffu - (uint32_t)(begin + i + j));
-                best = c > best ? c : best;
-            }
-            uint4 o = make_uint4(k[0] | (k[1] << 16), k[2] | (k[3] << 16), k[4] | (k[5] << 16), k[6] | (k[7] << 16));
-            *reinterpret_cast<uint4*>(keys + i) = o;
-        }
-    }
-    for (int i = vec_end + threadIdx.x; i < n; i += blockDim.x) {
-        const uint32_t k = key_of(s16[i]);
-        keys[i] = (uint16_t)k;
-        const unsigned long long c = ((unsigned long long)k << 32) | (0xffffffffu - (uint32_t)(begin + i));
+    stage_keys(reinterpret_cast<const uint16_t*>(src), n, keys, [&](uint32_t k, int i) {
+        const unsigned long long c = pair_of(k, begin + i);
         best = c > best ? c : best;
-    }
+    });
     best = block_max_u64(best, scratch);
     if (threadIdx.x == 0) cta_max = best;
     cluster.sync();
@@ -129,16 +108,9 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
         }
         merge_hist(cluster, h_cnt_hi, merged);
         select_bin(merged, 0, (double)k, &sel_bin, &sel_above);
-        const uint32_t hi = (uint32_t)sel_bin;
         const unsigned long long above = sel_above;
-        for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
-            const int i = i0 + (threadIdx.x & 31);
-            const uint32_t key = i < n ? keys[i] : 0u;
-            warp_hist_add(h_cnt_lo, i < n && (key >> 8) == hi, key & 255, 1ull);
-        }
-        merge_hist(cluster, h_cnt_lo, merged);
-        select_bin(merged, above, (double)k, &sel_bin, &sel_above);
-        thr = (hi << 8) | (uint32_t)sel_bin;
+        thr = select_low_byte(cluster, keys, n, (uint32_t)sel_bin, above, merged, h_cnt_lo, (double)k,
+                              [](uint32_t) { return true; }, [](uint32_t, bool) { return 1ull; }, &sel_bin, &sel_above).tau;
     }
 
     // ---- top-p threshold over the survivors
@@ -166,17 +138,11 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
         __syncthreads();
         const double target = (double)p * (double)scratch[0];
         select_bin(merged, 0, target, &sel_bin, &sel_above);
-        const uint32_t hi = (uint32_t)sel_bin;
         const unsigned long long above = sel_above;
-        for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
-            const int i = i0 + (threadIdx.x & 31);
-            const uint32_t key = i < n ? keys[i] : 0u;
-            const bool in = i < n && (key >> 8) == hi && key >= thr;
-            warp_hist_add(h_mass_lo, in, key & 255, in ? mass(key) : 0ull);
-        }
-        merge_hist(cluster, h_mass_lo, merged);
-        select_bin(merged, above, target, &sel_bin, &sel_above);
-        const uint32_t tp = (hi << 8) | (uint32_t)sel_bin;
+        const uint32_t tp = select_low_byte(cluster, keys, n, (uint32_t)sel_bin, above, merged, h_mass_lo, target,
+                                            [&](uint32_t key) { return key >= thr; },
+                                            [&](uint32_t key, bool in) { return in ? mass(key) : 0ull; }, &sel_bin,
+                                            &sel_above).tau;
         thr = tp > thr ? tp : thr;
     }
 
@@ -236,37 +202,6 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     cluster.sync();                                                   // peers' shared memory stays valid until rank 0 has read it
 }
 
-template <typename T>
-int launch(const void* logits, int64_t rows, int V, int64_t row_stride, int64_t vocab_offset, const float* temperature,
-           const int32_t* top_k, const float* top_p, const int64_t* seed, const int32_t* pos, int64_t* out_tokens,
-           float* out_pairs, cudaStream_t stream) {
-    const int C = cluster_size(rows, V);
-    const int slice = ((V + C - 1) / C + 7) & ~7;
-    const size_t smem = (size_t)slice * sizeof(uint16_t);
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(sample_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSliceBytes);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(rows * C));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, sample_kernel<T>, (const T*)logits, row_stride, V, vocab_offset, slice,
-                                       temperature, top_k, top_p, seed, pos, out_tokens, out_pairs);
-    if (e != cudaSuccess) {
-        set_error("sample_tokens: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return check_launch("sample_tokens");
-}
-
 }  // namespace
 }  // namespace sllm
 
@@ -278,7 +213,7 @@ extern "C" int sllm_sample_tokens(const void* logits, int64_t num_rows, int voca
     SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "sample_tokens: unsupported dtype tag %d", (int)dtype);
     SLLM_REQUIRE(num_rows >= 0 && num_rows <= (1 << 20), "sample_tokens: num_rows %lld out of range", (long long)num_rows);
     SLLM_REQUIRE(vocab_size > 0, "sample_tokens: vocab_size must be positive, got %d", vocab_size);
-    SLLM_REQUIRE(((int64_t)(vocab_size + kMaxCluster - 1) / kMaxCluster + 7) / 8 * 8 * 2 <= kMaxSliceBytes,
+    SLLM_REQUIRE(slice_fits(vocab_size, kMaxCluster, kKeyBytes, kKeyAlign),
                  "sample_tokens: vocab_size %d does not fit the shared memory of a %d-CTA cluster", vocab_size, kMaxCluster);
     SLLM_REQUIRE(vocab_offset >= 0 && vocab_offset + vocab_size <= (1 << 24),
                  "sample_tokens: global vocabulary indices must stay below 2^24 (vocab_offset %lld)", (long long)vocab_offset);
@@ -286,6 +221,9 @@ extern "C" int sllm_sample_tokens(const void* logits, int64_t num_rows, int voca
                  (long long)logits_row_stride, vocab_size);
     if (num_rows == 0) return 0;
     SLLM_REQUIRE(logits && temperature && top_k && top_p && seed && pos && out_tokens, "sample_tokens: null pointer");
-    SLLM_DISPATCH_DTYPE(dtype, return launch<T>(logits, num_rows, vocab_size, logits_row_stride, vocab_offset, temperature,
-                                                top_k, top_p, seed, pos, out_tokens, out_pairs, (cudaStream_t)stream));
+    const ClusterGeometry g = cluster_geometry(num_rows, vocab_size, kKeyBytes, kKeyAlign);
+    SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<sample_kernel<T>>(
+                                   num_rows, g.C, (size_t)g.slice * kKeyBytes, (cudaStream_t)stream, "sample_tokens",
+                                   (const T*)logits, logits_row_stride, vocab_size, vocab_offset, g.slice, temperature, top_k,
+                                   top_p, seed, pos, out_tokens, out_pairs));
 }

@@ -108,20 +108,11 @@ class LlamaPostLayer:
         sp, n = infer_state.sampling, infer_state.logprobs
         pen = sp is not None and sp.penalized
         sampled = sp is not None and sp.sampled
-        if not self.sharded:
-            if self.keep_logits:
-                self.last_logits = logits.clone() if pen else logits
-            chosen = self._penalised(logits, infer_state, idx, copy=n is not None) if pen else logits
-            if sampled:
-                tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
-            else:
-                tokens = torch.argmax(chosen, dim=1)
-            return tokens if n is None else (tokens,) + token_logprobs(logits, tokens, n)
-
         B, Vs = logits.shape
-        if (sp is not None and sp.filtered) or n is not None:
-            # top-k / top-p and log-probabilities need whole rows: gather them, choose the token on every rank
-            full = self._gather_logits(logits)
+        if not self.sharded or (sp is not None and sp.filtered) or n is not None:
+            # choose the token from whole rows: top-k / top-p and log-probabilities need them, so a sharded lm_head gathers
+            # them and every rank chooses the token
+            full = self._gather_logits(logits) if self.sharded else logits
             if self.keep_logits:
                 self.last_logits = full.clone() if pen else full
             chosen = self._penalised(full, infer_state, idx, copy=n is not None) if pen else full
