@@ -62,31 +62,38 @@ class BlockManager:
                                  seq_ids_list=None, target_lens_list=None, want_new_blocks: bool = True) -> torch.Tensor:
         """Make sure seq #i has ceil(target_lens[i] / block_size) blocks.  Returns the new block ids (int64,
         batch order), like the reference (useful for swapping).  Pass the host lists to avoid a device sync."""
-        sids = self._to_list(seq_ids, seq_ids_list)
-        lens = self._to_list(target_lens, target_lens_list)
-        idx = np.asarray(sids, dtype=np.int64)
-        target = (np.asarray(lens, dtype=np.int64) + (self.block_size - 1)) // self.block_size
-        have = self._host_nsab[idx] if len(sids) else np.zeros((0,), dtype=np.int64)
+        total = self.reserve_blocks_for_seqs(self._to_list(seq_ids, seq_ids_list), self._to_list(target_lens, target_lens_list))
+        new_blocks = torch.empty((total,), dtype=torch.int64, device=self.block_table.device) if want_new_blocks else None
+        if total > 0:
+            self.allocate_reserved_blocks(seq_ids.to(torch.int32).contiguous(), target_lens.to(torch.int32).contiguous(),
+                                          new_blocks)
+        return new_blocks
+
+    def reserve_blocks_for_seqs(self, seq_ids_list, target_lens_list) -> int:
+        """Host half of allocate_blocks_for_seqs: count ceil(target_lens_list[i] / block_size) blocks for seq #i into the host
+        mirror and `num_free_blocks`, and return how many are new.  Raises RuntimeError, changing nothing, when a sequence would
+        need more than max_blocks_per_seq blocks or the free blocks do not suffice; the caller then enqueues nothing."""
+        idx = np.asarray(seq_ids_list, dtype=np.int64)
+        target = (np.asarray(target_lens_list, dtype=np.int64) + (self.block_size - 1)) // self.block_size
+        have = self._host_nsab[idx]
         assert (have <= target).all(), \
             f"(On {self.device_name}) Logic error: Some sequences have more blocks already allocated than needed."
-        if len(sids) and int(target.max()) > self.max_blocks_per_seq:
+        if len(idx) and int(target.max()) > self.max_blocks_per_seq:
             raise RuntimeError(f"sequence needs {int(target.max())} blocks > max_blocks_per_seq={self.max_blocks_per_seq}")
         total = int((target - have).sum())
         if total > self.num_free_blocks:
             raise RuntimeError(f"No enough free blocks available on {self.device_name} ({self.num_blocks} in total, "
                                f"{self.num_free_blocks} free, {total} requested)")
-        new_blocks = torch.empty((total,), dtype=torch.int64, device=self.block_table.device) if want_new_blocks else None
-        if len(sids) and total > 0:
-            if seq_ids.dtype != torch.int32:
-                seq_ids = seq_ids.to(torch.int32)
-            if target_lens.dtype != torch.int32:
-                target_lens = target_lens.to(torch.int32)
-            _allocate_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free,
-                             seq_ids.contiguous(), target_lens.contiguous(), self.block_size,
-                             new_blocks if (want_new_blocks and total > 0) else None, self._status)
-            self._host_nsab[idx] = target
-            self.num_free_blocks -= total
-        return new_blocks
+        self._host_nsab[idx] = target
+        self.num_free_blocks -= total
+        return total
+
+    def allocate_reserved_blocks(self, seq_ids: torch.Tensor, target_lens: torch.Tensor, new_blocks=None):
+        """Device half of allocate_blocks_for_seqs: one launch of the allocation kernel on this manager's tables, for blocks
+        reserve_blocks_for_seqs has counted (int32 contiguous ids and lengths; new ids into `new_blocks` when given).  No host
+        work, so a CUDA graph can capture it with static ids and lengths and reserve before each replay."""
+        _allocate_kernel(self.num_seq_allocated_blocks, self.block_table, self.is_block_free, seq_ids, target_lens,
+                         self.block_size, new_blocks, self._status)
 
     def fork_blocks_for_seqs(self, src_seq_ids: torch.Tensor, dst_seq_ids: torch.Tensor, lens: torch.Tensor, *,
                              src_seq_ids_list, dst_seq_ids_list, lens_list):
@@ -221,3 +228,7 @@ class BlockManager:
 
     def get_num_allocated_blocks_host(self, seq_ids_list) -> list:
         return self._host_nsab[np.asarray(seq_ids_list, dtype=np.int64)].tolist()
+
+    def get_num_shared_blocks_host(self, seq_ids_list) -> list:
+        """Leading blocks each sequence shares with a fork (host mirror, no sync)."""
+        return self._host_shared[np.asarray(seq_ids_list, dtype=np.int64)].tolist()

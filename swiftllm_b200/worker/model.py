@@ -113,7 +113,7 @@ class LlamaModel:
         self.cpu_block_manager = self.gpu_block_manager = None
         self.tp_group = None
         self._graphs = {}
-        # pinned staging ring for per-step metadata (eager path): a slot is rewritten only after the H2D copy that last read it
+        # pinned staging ring for per-step metadata (every step path): a slot is rewritten only after the H2D copy that last read it
         # has completed (event per slot), so back-to-back forward_async calls never race the copy engine
         self._stage_ring = []
         self._stage_next = 0
@@ -295,18 +295,63 @@ class LlamaModel:
             torch.cuda.current_stream().wait_event(self._swap_done)
             self._swap_done = None
 
-    def _stage_metadata(self, *parts):
-        """One persistent pinned host buffer (ring of slots), one async H2D copy; returns int32 device views (one per list)."""
-        flat = np.fromiter(itertools.chain(*parts), dtype=np.int32)
-        host, ev = self._stage_slot(flat.size)
-        host[:flat.size].numpy()[:] = flat
-        dev = host[:flat.size].to(self.device, non_blocking=True)
+    def _stage_metadata(self, *parts, out: Optional[torch.Tensor] = None):
+        """One persistent pinned host buffer (ring of slots), one async H2D copy; returns int32 device views (one per list), or
+        with `out` (a graph's static buffer of exactly that size) copies into it and returns None."""
+        n = sum(len(p) for p in parts)
+        host, ev = self._stage_slot(n)
+        hv, off = host.numpy(), 0
+        for p in parts:
+            hv[off:off + len(p)] = p
+            off += len(p)
+        if out is not None:
+            out.copy_(host[:n], non_blocking=True)
+            ev.record()
+            return None
+        dev = host[:n].to(self.device, non_blocking=True)
         ev.record()
         views, off = [], 0
         for p in parts:
             views.append(dev[off:off + len(p)])
             off += len(p)
         return views
+
+    def _infer_state(self, ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, *, max_prefill_len: int, max_decoding_len: int,
+                     decoding_lens: Optional[list], prefix=None, max_prefill_kv_len: int = 0, speculative: bool = False,
+                     ignore_kvcache: bool = False, words=None, filtered: bool = False, sampled: bool = True, sampling_pos=None,
+                     top_n: Optional[int] = None, prompt_state: Optional[PromptLogprobsState] = None, block_table=None,
+                     token_cache=None) -> LlamaInferState:
+        """The LlamaInferState of a step from its int32 device views (input ids, block-table rows, sequence lengths with the
+        prefill entries first, prompt lengths and first rows, positions, rows to sample) and the sizes the host knows; the batch
+        counts are the views' shapes.  decoding_lens: host decode lengths for the reference's split heuristic, None in a graph
+        captured for a length bucket (the largest split).  prefix: first position of each chunk (chunked prefill, speculative
+        verification), with max_prefill_kv_len.  words: staged sampling_params.sampling_words, noise counter `sampling_pos`
+        (default: the sequence lengths); with penalties the sampling state also carries the token history: the input ids, the
+        block table and the token pages (default: the model's)."""
+        mc = self.model_config
+        B, T, P = seq_ids.shape[0], ids.shape[0], p_lens.shape[0]
+        num_prefill_tokens = T - (B - P)
+        sampling = None
+        if words is not None:
+            sampling = SamplingState.from_staged(words, seq_lens if sampling_pos is None else sampling_pos, filtered, sampled)
+            if sampling.penalized:
+                sampling = dataclasses.replace(
+                    sampling, input_ids=ids, block_table=self.gpu_block_manager.block_table if block_table is None else block_table,
+                    token_cache=self.token_cache if token_cache is None else token_cache)
+        sbs = 2048 if decoding_lens is None else select_seq_block_size(mc.num_kv_heads, decoding_lens, max_decoding_len)
+        return LlamaInferState(
+            batch_size=B, num_tokens=T, seq_ids=seq_ids, softmax_scale=mc.head_dim ** -0.5,
+            num_prefill_seqs=P, num_prefill_tokens=num_prefill_tokens, prefill_seq_start_locs=p_starts,
+            # ends at num_prefill_tokens (the reference puts num_tokens there, model.py:336-339, which over-declares
+            # the last prompt by the number of decoding tokens on mixed batches; SURVEY.md §3.1)
+            prefill_seq_start_locs_with_end=torch.cat([p_starts, p_starts.new_tensor([num_prefill_tokens])]) if P > 0 else p_starts,
+            prefill_seq_lens=p_lens, max_prefill_len=max_prefill_len,
+            num_decoding_seqs=B - P, decoding_seq_lens=seq_lens[P:], max_decoding_len=max_decoding_len,
+            seq_block_size=sbs, num_seq_blocks=(max_decoding_len + sbs - 1) // sbs,
+            position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
+            ignore_kvcache=ignore_kvcache, paged_attn_seq_block_size=0, last_token_indices=last,
+            prefill_prefix_lens=prefix, max_prefill_kv_len=max_prefill_kv_len, speculative=speculative,
+            sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state)
 
     @torch.inference_mode()
     def forward(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
@@ -472,7 +517,6 @@ class LlamaModel:
         if B == 0:
             return []
         self._check_shared_writes(seq_ids_list, prefix)
-        mc = self.model_config
         T = sum(rows)
         rep = np.repeat(np.arange(B), rows)
         flat_ids = list(itertools.chain(*input_ids_list))
@@ -488,21 +532,13 @@ class LlamaModel:
         views = self._stage_metadata(*([row_words] if samp else []), flat_ids, seq_ids_list, seq_lengths, rows, starts,
                                      positions, range(T), prefix, row_pos)
         ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, p_prefix, r_pos = views[-9:]
-        sampling = SamplingState.from_staged(views[0], r_pos, samp[1]) if samp else None
         bm = self.gpu_block_manager
         bm.allocate_blocks_for_seqs(seq_ids, seq_lens, seq_ids_list=seq_ids_list, target_lens_list=seq_lengths,
                                     want_new_blocks=False)
-        infer_state = LlamaInferState(
-            batch_size=B, num_tokens=T, seq_ids=seq_ids, softmax_scale=mc.head_dim ** -0.5,
-            num_prefill_seqs=B, num_prefill_tokens=T, prefill_seq_start_locs=p_starts,
-            prefill_seq_start_locs_with_end=torch.cat([p_starts, p_starts.new_tensor([T])]),
-            prefill_seq_lens=p_lens, max_prefill_len=max(rows),
-            num_decoding_seqs=0, decoding_seq_lens=seq_lens[B:], max_decoding_len=0,
-            seq_block_size=select_seq_block_size(mc.num_kv_heads, [], 0), num_seq_blocks=0,
-            position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-            ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last,
-            prefill_prefix_lens=p_prefix, max_prefill_kv_len=max(seq_lengths), sampling=sampling, speculative=True,
-        )
+        infer_state = self._infer_state(ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, max_prefill_len=max(rows),
+                                        max_decoding_len=0, decoding_lens=[], prefix=p_prefix,
+                                        max_prefill_kv_len=max(seq_lengths), speculative=True,
+                                        words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampling_pos=r_pos)
         tokens = self._forward(ids, infer_state).tolist()
         out, keep = [], []
         for ids_i, s, n_rows, p in zip(input_ids_list, starts, rows, prefix):
@@ -526,7 +562,6 @@ class LlamaModel:
         `prompt_plan` (forward_with_logprobs._prompt_plan, some rows to score): (that, (prompt logprobs, ranks, top ids, top
         logprobs)).  The step stages exactly what it stages without one: the post layer builds the rows and targets on the device
         after the layers, so nothing of the prompt part is allocated while the forward's activations are."""
-        mc = self.model_config
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
@@ -573,44 +608,26 @@ class LlamaModel:
         pp = prompt_plan
         prompt_state = None if pp is None else PromptLogprobsState(
             pieces=pp["pieces"], num_rows=pp["num_rows"], input_ids=ids, top_n=pp["top_n"], block_rows=self._prompt_block_rows())
-        sampling = SamplingState.from_staged(views[0], seq_lengths, samp[1]) if samp else None
-        if penalized:
-            sampling = dataclasses.replace(sampling, sampled=sampled, input_ids=ids,
-                                           block_table=self.gpu_block_manager.block_table, token_cache=self.token_cache)
-            self._penalties_used = True
+        self._penalties_used |= penalized
 
         if not ignore_kvcache:
             self.gpu_block_manager.allocate_blocks_for_seqs(seq_ids, seq_lengths, seq_ids_list=seq_ids_list,
                                                             target_lens_list=seq_lengths_list, want_new_blocks=False)
 
-        seq_block_size = select_seq_block_size(mc.num_kv_heads, list(decoding_seq_lens_list), max_decoding_len)
-        infer_state = LlamaInferState(
-            batch_size=batch_size, num_tokens=num_tokens,
-            seq_ids=seq_ids, softmax_scale=mc.head_dim ** -0.5,
-            num_prefill_seqs=num_prefill_seqs, num_prefill_tokens=num_prefill_tokens,
-            prefill_seq_start_locs=p_starts,
-            # ends at num_prefill_tokens (the reference puts num_tokens there, model.py:336-339, which over-declares
-            # the last prompt by the number of decoding tokens on mixed batches; SURVEY.md §3.1)
-            prefill_seq_start_locs_with_end=torch.cat([p_starts, p_starts.new_tensor([num_prefill_tokens])])
-            if num_prefill_seqs > 0 else p_starts,
-            prefill_seq_lens=p_lens, max_prefill_len=max_prefill_len,
-            num_decoding_seqs=batch_size - num_prefill_seqs, decoding_seq_lens=seq_lengths[num_prefill_seqs:],
-            max_decoding_len=max_decoding_len,
-            seq_block_size=seq_block_size, num_seq_blocks=(max_decoding_len + seq_block_size - 1) // seq_block_size,
-            position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-            ignore_kvcache=ignore_kvcache,
-            paged_attn_seq_block_size=0, last_token_indices=last,
-            prefill_prefix_lens=p_prefix if chunked else None,
-            max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0,
-            sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state,
-        )
+        infer_state = self._infer_state(
+            ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, max_prefill_len=max_prefill_len,
+            max_decoding_len=max_decoding_len, decoding_lens=list(decoding_seq_lens_list), prefix=p_prefix if chunked else None,
+            max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0, ignore_kvcache=ignore_kvcache,
+            words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampled=sampled, top_n=top_n,
+            prompt_state=prompt_state)
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
     def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
                               sampled=True):
-        """Pure-decode step replayed from a CUDA graph.  Static device buffers hold the step's metadata; the graph
-        (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
+        """Pure-decode step replayed from a CUDA graph.  The step's metadata is staged through the same pinned ring as an eager
+        step's, into the graph's static device buffer, and its blocks are reserved on the manager's host mirror like an eager
+        step's; the graph (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
         allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
         filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy.  A step
         with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
@@ -641,31 +658,10 @@ class LlamaModel:
                 self._graphs.pop(next(iter(self._graphs)))
             g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled)
         self._graphs[key] = g                    # (re)insert as most recently used
-        # host-side bookkeeping of the allocator (exhaustion check + mirror), no device work here
-        bm = self.gpu_block_manager
-        idx = np.asarray(seq_ids_list, dtype=np.int64)
-        target = (np.asarray(lens_list, dtype=np.int64) + bm.block_size - 1) // bm.block_size
-        have = bm._host_nsab[idx]
-        assert (have <= target).all()
-        total = int((target - have).sum())
-        if total > bm.num_free_blocks:
-            raise RuntimeError(f"No enough free blocks available on GPU ({bm.num_blocks} in total, "
-                               f"{bm.num_free_blocks} free, {total} requested)")
-        bm._host_nsab[idx] = target
-        bm.num_free_blocks -= total
-        # pinned staging: a ring of (buffer, event) pairs per graph; a buffer is rewritten only after the H2D copy that last
-        # read it has finished, so back-to-back forward_async calls are safe
-        i = g["next"]; g["next"] = (i + 1) % len(g["host"])
-        host, ev = g["host"][i]
-        ev.synchronize()
-        hv = host.numpy()
-        if samp:
-            nw = len(samp[0])                   # 5 * B sampling words, 8 * B with penalties
-            hv[:nw] = samp[0]
-            hv = hv[nw:]
-        hv[:B] = flat_ids; hv[B:2 * B] = seq_ids_list; hv[2 * B:3 * B] = lens_list
-        g["meta"].copy_(host, non_blocking=True)
-        ev.record()
+        # the blocks are counted on the host, and the eager step's errors raised, before anything is enqueued; the graph's
+        # allocation kernel hands them out
+        self.gpu_block_manager.reserve_blocks_for_seqs(seq_ids_list, lens_list)
+        self._stage_metadata(*([samp[0]] if samp else []), flat_ids, seq_ids_list, lens_list, out=g["meta"])
         self._wait_for_swaps()
         self._penalties_used |= penalized
         g["graph"].replay()
@@ -679,32 +675,24 @@ class LlamaModel:
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
         also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
         the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax."""
-        from swiftllm_b200.worker.kernels.block_mgmt import allocate_blocks_for_seqs as alloc_kernel
-        mc, ec = self.model_config, self.engine_config
+        ec = self.engine_config
         dev = self.device
         nw = 0 if filtered is None else (8 if penalized else 5) * B
         meta = torch.zeros((nw + 3 * B,), dtype=torch.int32, device=dev)
-        host = [(torch.zeros((nw + 3 * B,), dtype=torch.int32).pin_memory(), torch.cuda.Event()) for _ in range(self._STAGE_SLOTS)]
         ids, seq_ids, lens = meta[nw:nw + B], meta[nw + B:nw + 2 * B], meta[nw + 2 * B:]
-        sampling = None if filtered is None else SamplingState.from_staged(meta[:nw], lens, filtered, sampled)
         last = torch.arange(B, dtype=torch.int32, device=dev)
         empty = torch.empty((0,), dtype=torch.int32, device=dev)
 
         def step(bm, k_cache, v_cache, token_cache):
-            samp_state = sampling if not penalized else \
-                dataclasses.replace(sampling, input_ids=ids, block_table=bm.block_table, token_cache=token_cache)
-            alloc_kernel(bm.num_seq_allocated_blocks, bm.block_table, bm.is_block_free, seq_ids, lens, bm.block_size,
-                         None, bm._status)
+            # the replayed lengths are unknown here: the kernel runs on every replay, reserve_blocks_for_seqs counts its blocks
+            bm.allocate_reserved_blocks(seq_ids, lens)
+            # `pos` is held until the step returns: the order in which a capture frees its tensors decides where later captures
+            # into the shared pool place theirs, and parity tests read post_layer.last_logits, the logits of the graph captured last
             pos = (lens - 1).long()
-            st = LlamaInferState(
-                batch_size=B, num_tokens=B, seq_ids=seq_ids, softmax_scale=mc.head_dim ** -0.5,
-                num_prefill_seqs=0, num_prefill_tokens=0, prefill_seq_start_locs=empty,
-                prefill_seq_start_locs_with_end=empty, prefill_seq_lens=empty, max_prefill_len=0,
-                num_decoding_seqs=B, decoding_seq_lens=lens, max_decoding_len=bucket_len,
-                seq_block_size=2048, num_seq_blocks=(bucket_len + 2047) // 2048,
-                position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
-                ignore_kvcache=False, paged_attn_seq_block_size=0, last_token_indices=last, sampling=samp_state,
-                logprobs=top_n)
+            st = self._infer_state(ids, seq_ids, lens, empty, empty, pos, last, max_prefill_len=0,
+                                   max_decoding_len=bucket_len, decoding_lens=None,
+                                   words=None if filtered is None else meta[:nw], filtered=filtered, sampled=sampled,
+                                   top_n=top_n, block_table=bm.block_table, token_cache=token_cache)
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
@@ -733,7 +721,7 @@ class LlamaModel:
         torch.cuda.synchronize()
         tokens, logprobs = (out, None) if top_n is None else (out[0], out[1:])
         # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph
-        return dict(graph=graph, meta=meta, host=host, next=0, tokens=tokens, logprobs=logprobs, keep=(last, empty))
+        return dict(graph=graph, meta=meta, tokens=tokens, logprobs=logprobs, keep=(last, empty))
 
     # ------------------------------------------------------------------ shared blocks
     def _check_shared_writes(self, seq_ids_list, first_positions):
@@ -743,13 +731,13 @@ class LlamaModel:
         bm = self.gpu_block_manager
         if not bm.forked or len(seq_ids_list) == 0:
             return
-        idx = np.asarray(seq_ids_list, dtype=np.int64)
+        shared = bm.get_num_shared_blocks_host(seq_ids_list)
         pos = np.asarray(first_positions, dtype=np.int64)
-        bad = pos // bm.block_size < bm._host_shared[idx]
+        bad = pos // bm.block_size < shared
         if bad.any():
             i = int(np.argmax(bad))
-            raise ValueError(f"sequence {int(idx[i])} would write position {int(pos[i])}, inside one of its first "
-                             f"{int(bm._host_shared[idx[i]])} blocks, which it shares with a fork: shared blocks are read-only")
+            raise ValueError(f"sequence {int(seq_ids_list[i])} would write position {int(pos[i])}, inside one of its first "
+                             f"{shared[i]} blocks, which it shares with a fork: shared blocks are read-only")
 
     @torch.inference_mode()
     def fork_seqs(self, src_seq_ids_list: list, dst_seq_ids_list: list, lens_list: list):
@@ -772,7 +760,7 @@ class LlamaModel:
             raise ValueError(f"fork_seqs: {B} sources but {len(dst_seq_ids_list)} destinations and {len(lens_list)} lengths")
         src, dst, lens = ([int(x) for x in l] for l in (src_seq_ids_list, dst_seq_ids_list, lens_list))
         gpu, cpu = self.gpu_block_manager, self.cpu_block_manager
-        bs, nseq = gpu.block_size, len(gpu._host_nsab)
+        bs, nseq = gpu.block_size, gpu.block_table.shape[0]
         for sid in src + dst:
             if not 0 <= sid < nseq:
                 raise ValueError(f"fork_seqs: sequence id {sid} outside [0, {nseq})")
@@ -780,15 +768,16 @@ class LlamaModel:
             raise ValueError("fork_seqs: a destination sequence repeats")
         if set(dst) & set(src):
             raise ValueError(f"fork_seqs: sequences {sorted(set(dst) & set(src))} are both a source and a destination")
-        for s, d, p in zip(src, dst, lens):
-            if cpu._host_nsab[s] > 0:
+        on_gpu, on_cpu = gpu.get_num_allocated_blocks_host(src + dst), cpu.get_num_allocated_blocks_host(src + dst)
+        for i, (s, d, p) in enumerate(zip(src, dst, lens)):
+            if on_cpu[i] > 0:
                 raise ValueError(f"fork_seqs: source sequence {s} is swapped out")
-            have = int(gpu._host_nsab[s])
+            have = on_gpu[i]
             if have == 0:
                 raise ValueError(f"fork_seqs: source sequence {s} holds no GPU blocks")
             if not 1 <= p <= have * bs:
                 raise ValueError(f"fork_seqs: length {p} outside [1, {have * bs}] for source sequence {s} ({have} blocks)")
-            if gpu._host_nsab[d] > 0 or cpu._host_nsab[d] > 0:
+            if on_gpu[B + i] > 0 or on_cpu[B + i] > 0:
                 raise ValueError(f"fork_seqs: destination sequence {d} already holds blocks")
         if B == 0:
             return

@@ -161,3 +161,23 @@ def test_block_manager_random_operation_sequences_match_the_oracle():
                 assert np.array_equal(bm.is_block_free.numpy(), ob.is_block_free) and bm.num_free_blocks == ob.num_free_blocks
                 for s in range(nseq):
                     assert np.array_equal(bm.block_table.numpy()[s, : n[s]], ob.block_table[s, : n[s]])
+
+
+def test_block_reservation_refuses_without_changing_anything():
+    """BlockManager.reserve_blocks_for_seqs, the host half with which every step path (eager, CUDA graph, speculative) counts its
+    blocks: it counts only the new blocks into the mirror and the free count, touches no device table, and a sequence past
+    max_blocks_per_seq or more new blocks than are free raises RuntimeError and changes nothing."""
+    from swiftllm_b200.worker.block_manager import BlockManager
+    import pytest
+    bm = BlockManager("GPU", 6, 4, 3, 16, device="cpu")
+    assert bm.reserve_blocks_for_seqs([0, 1], [40, 1]) == 4
+    assert bm._host_nsab.tolist() == [3, 1, 0, 0] and bm.num_free_blocks == 2
+    assert bm.reserve_blocks_for_seqs([0, 1], [48, 16]) == 0                   # already held
+    assert bm.reserve_blocks_for_seqs([], []) == 0
+    before = bm._host_nsab.copy()
+    with pytest.raises(RuntimeError, match=r"^sequence needs 4 blocks > max_blocks_per_seq=3$"):
+        bm.reserve_blocks_for_seqs([2, 0], [16, 49])
+    with pytest.raises(RuntimeError, match=r"^No enough free blocks available on GPU \(6 in total, 2 free, 4 requested\)$"):
+        bm.reserve_blocks_for_seqs([2, 3], [16, 48])
+    assert np.array_equal(bm._host_nsab, before) and bm.num_free_blocks == 2
+    assert not bm.num_seq_allocated_blocks.any() and bool(bm.is_block_free.all())

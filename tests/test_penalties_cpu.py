@@ -480,3 +480,35 @@ def test_sharded_lm_head_penalties_equal_the_unsharded_tokens(world, filtered):
         assert p.exitcode == 0
     assert all(ok for ok, _ in out), out
     assert all(t == out[0][1] for _, t in out)
+
+
+def test_steps_choose_tokens_with_the_sampling_kernel_unless_every_penalised_row_is_greedy():
+    """What the post layer is handed on eager steps (forward and forward_with_logprobs, over random parameter lists): no sampling
+    state for an all-greedy list without penalties, the argmax of penalised logits (sampled False) only when some row has penalties
+    and every temperature is 0, and the sampling kernel (sampled True) on every other list."""
+    from cpu_shim import product_on_cpu
+    from oracle.model import OracleWeights
+    from test_host_path_cpu import CFG, _product
+    from test_sampling_cpu import _record_sampling
+    from swiftllm_b200 import SamplingParams
+    w = OracleWeights.random(CFG, dtype=torch.float16, seed=7, std=0.08)
+    rng = np.random.default_rng(11)
+    with product_on_cpu(PATCH):
+        m = _product(w)
+        _record_sampling(m)
+        seen = set()
+        for k in range(24):
+            sp = [SamplingParams(float(rng.choice([0.0, 0.0, 0.7])), logprobs=int(rng.integers(0, 3)) if rng.random() < 0.5 else None,
+                                 seed=int(rng.integers(0, 100)),
+                                 repetition_penalty=1.3 if rng.random() < 0.3 else 1.0) for _ in range(2)]
+            call = m.forward_with_logprobs if k % 2 else m.forward
+            call([[1, 2, 3], [4, 5]], [0, 1], [], sampling_params_list=sp)
+            st = m._last_sampling
+            greedy, penalised = all(s.temperature == 0 for s in sp), any(s.has_penalties() for s in sp)
+            if greedy and not penalised:
+                assert st is None
+            else:
+                assert st.sampled == (not greedy) and st.penalized == penalised
+            seen.add((greedy, penalised))
+            m.free_seqs_resources([0, 1])
+        assert seen == {(False, False), (False, True), (True, False), (True, True)}
