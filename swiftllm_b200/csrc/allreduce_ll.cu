@@ -23,18 +23,16 @@
 // deadlock as long as each GPU dispatches CTAs in increasing blockIdx order: grid and row-to-CTA map are the same on every rank,
 // so in all three phases CTA c waits only for CTA c of each peer, and the lowest CTA index still unfinished anywhere is then
 // resident on every rank where it has not finished.
-#include <type_traits>
-
-#include "common.cuh"
+// Peer loads, multimem.st, the epoch step and the host checks / launch are shared with allreduce_norm.cu (exchange.cuh); the
+// add + RMSNorm row epilogue with rmsnorm_kernel (common.cuh).
+#include "exchange.cuh"
 
 namespace sllm {
 
-constexpr int LL_MAX_RANKS = 8;
-
 struct LlParams {
     const void* partial;                    // this rank's partial [T, H], plain (local)
-    void* rs_recv[LL_MAX_RANKS];            // rs_recv of every rank (peer-mapped): [N src][rows_per_rank][H] in LL format (2x bytes)
-    void* ag_recv[LL_MAX_RANKS];            // ag_recv of every rank (peer-mapped): [max_tokens][H] in LL format
+    void* rs_recv[MAX_RANKS];               // rs_recv of every rank (peer-mapped): [N src][rows_per_rank][H] in LL format (2x bytes)
+    void* ag_recv[MAX_RANKS];               // ag_recv of every rank (peer-mapped): [max_tokens][H] in LL format
     void* mc_ag_recv;                       // multicast address of ag_recv, or NULL
     void* x_out;                            // local plain [T, H]
     void* residual; const void* weight;
@@ -47,22 +45,13 @@ struct LlParams {
 __device__ __forceinline__ void st_ll(void* p, uint32_t w0, uint32_t w1, uint32_t tag) {
     asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(w0), "r"(tag), "r"(w1), "r"(tag) : "memory");
 }
-__device__ __forceinline__ void multimem_st_ll(void* mc, uint32_t w0, uint32_t w1, uint32_t tag) {
-    // a store moves bits: the (validated) bf16x2 vector form of multimem.st carries the four 32-bit words unchanged
-    asm volatile("multimem.st.relaxed.sys.global.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(mc), "r"(w0), "r"(tag), "r"(w1), "r"(tag) : "memory");
-}
-__device__ __forceinline__ uint4 ld_ll(const void* p) {
-    uint4 u;
-    asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(p) : "memory");
-    return u;
-}
 // `u` = a first (possibly stale) read of the line at p: spin until both 8-byte units of the 16-byte line carry `tag`.
 // Callers issue the first reads of ALL their lines before calling this, so the loads are in flight together.
 __device__ __forceinline__ uint4 poll_ll(const void* p, uint4 u, uint32_t tag, int rank, int what) {
     uint32_t spins = 0;
     while (u.y != tag || u.w != tag) {
         if (++spins > (1u << 26)) { printf("sllm: LL exchange watchdog (rank %d, phase %d, tag %u, saw %u/%u)\n", rank, what, tag, u.y, u.w); __trap(); }
-        u = ld_ll(p);
+        u = ld_peer(p);
     }
     return u;
 }
@@ -71,7 +60,6 @@ template <typename T, bool NVLS>
 __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_ll_kernel(const LlParams p) {
     extern __shared__ uint4 row_smem[];
     __shared__ float red[16];
-    using TT = Traits<T>;
     const int nvec = p.hidden >> 3;                                  // 16-byte plain vectors per row; LL: 2 lines of 16 B each
     const uint32_t e = p.epoch[p.slot] + 1;
     const int64_t ll_row = (int64_t)p.hidden * 4;                    // bytes of one row in LL format
@@ -101,17 +89,17 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_ll_kernel(const LlP
             float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             // first reads of every source's two lines are issued back to back (independent loads in flight); late lines are
             // re-polled when their turn comes.  Accumulation in fixed rank order, fp32: the same sum as the other kernels.
-            uint4 la[LL_MAX_RANKS], lb[LL_MAX_RANKS];
+            uint4 la[MAX_RANKS], lb[MAX_RANKS];
 #pragma unroll
-            for (int r = 0; r < LL_MAX_RANKS; r++) {
+            for (int r = 0; r < MAX_RANKS; r++) {
                 if (r < N && r != me) {
                     const char* q = rbase + (int64_t)r * p.rows_per_rank * ll_row + 32 * i;
-                    la[r] = ld_ll(q); lb[r] = ld_ll(q + 16);
+                    la[r] = ld_peer(q); lb[r] = ld_peer(q + 16);
                 }
             }
             const Vec8<T> own = ld_vec8(mine + 8 * i);
 #pragma unroll
-            for (int r = 0; r < LL_MAX_RANKS; r++) {
+            for (int r = 0; r < MAX_RANKS; r++) {
                 if (r < N) {
                     Vec8<T> v;
                     if (r == me) {
@@ -122,46 +110,32 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_ll_kernel(const LlP
                         const uint4 u = make_uint4(x.x, x.z, y.x, y.z);
                         v = *reinterpret_cast<const Vec8<T>*>(&u);
                     }
-#pragma unroll
-                    for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(v.v[j]); acc[2 * j] += f.x; acc[2 * j + 1] += f.y; }
+                    acc_f32(acc, v);
                 }
             }
-            Vec8<T> a, b = ld_vec8(rr + 8 * i);
+            Vec8<T> sum;
 #pragma unroll
-            for (int j = 0; j < 4; j++) a.v[j] = __hadd2_rn(TT::from_f2(make_float2(acc[2 * j], acc[2 * j + 1])), b.v[j]);   // h(h(sum) + r)
-            st_vec8(rr + 8 * i, a);
-            row_smem[i] = *reinterpret_cast<uint4*>(&a);
-#pragma unroll
-            for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(a.v[j]); ss += f.x * f.x + f.y * f.y; }
+            for (int j = 0; j < 4; j++) sum.v[j] = Traits<T>::from_f2(make_float2(acc[2 * j], acc[2 * j + 1]));
+            add_residual(sum, rr + 8 * i, &row_smem[i], ss);
         }
         ss = warp_sum(ss);
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
         __syncthreads();                                             // red[] of the previous row fully consumed
-        if (lane == 0) red[warp] = ss;
-        __syncthreads();
-        float total = 0.f;
-        for (int w = 0; w < nwarps; w++) total += red[w];
-        const float rstd = 1.0f / sqrtf(total / (float)p.hidden + p.eps);
+        const float rstd = row_rstd(ss, red, p.hidden, p.eps);
         const T* wt = reinterpret_cast<const T*>(p.weight);
         T* xo = reinterpret_cast<T*>(p.x_out) + (int64_t)t * p.hidden;
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-            Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
-            Vec8<T> w = ld_vec8(wt + 8 * i);
+            const Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
             Vec8<T> o;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                float2 f = TT::to_f2(a.v[j]), g = TT::to_f2(w.v[j]);
-                o.v[j] = TT::from_f2(make_float2((f.x * rstd) * g.x, (f.y * rstd) * g.y));
-            }
+            rms_scale(o, a, rstd, wt + 8 * i);
             st_vec8(xo + 8 * i, o);                                  // my own copy: plain
             const uint4 u = *reinterpret_cast<const uint4*>(&o);
             const int64_t off = (int64_t)t * ll_row + 32 * i;
             if constexpr (NVLS) {                                    // the switch replicates the line into every rank's ag_recv
-                multimem_st_ll(reinterpret_cast<char*>(p.mc_ag_recv) + off, u.x, u.y, e);
-                multimem_st_ll(reinterpret_cast<char*>(p.mc_ag_recv) + off + 16, u.z, u.w, e);
+                multimem_st(reinterpret_cast<char*>(p.mc_ag_recv) + off, u.x, e, u.y, e);
+                multimem_st(reinterpret_cast<char*>(p.mc_ag_recv) + off + 16, u.z, e, u.w, e);
             } else {
 #pragma unroll
-                for (int k = 1; k < LL_MAX_RANKS; k++) {             // start with the next rank: owners do not all hit one target
+                for (int k = 1; k < MAX_RANKS; k++) {                // start with the next rank: owners do not all hit one target
                     if (k < N) {
                         int r = me + k;
                         if (r >= N) r -= N;
@@ -180,18 +154,13 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_ll_kernel(const LlP
         const char* src = reinterpret_cast<const char*>(p.ag_recv[me]) + (int64_t)t * ll_row;
         T* xo = reinterpret_cast<T*>(p.x_out) + (int64_t)t * p.hidden;
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-            uint4 a = ld_ll(src + 32 * i), b = ld_ll(src + 32 * i + 16);
+            uint4 a = ld_peer(src + 32 * i), b = ld_peer(src + 32 * i + 16);
             a = poll_ll(src + 32 * i, a, e, me, 3); b = poll_ll(src + 32 * i + 16, b, e, me, 3);
             *reinterpret_cast<uint4*>(xo + 8 * i) = make_uint4(a.x, a.z, b.x, b.z);
         }
     }
 
-    // ---- the last CTA to finish advances the epoch (every CTA has read it by then)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t* done = p.epoch + 16 + p.slot;
-        if (atomicAdd(done, 1u) == gridDim.x - 1) { *done = 0; __threadfence(); p.epoch[p.slot] = e; }
-    }
+    advance_epoch(p.epoch, p.slot, e);
 }
 
 }  // namespace sllm
@@ -206,9 +175,7 @@ extern "C" int sllm_allreduce_add_rmsnorm_ll(const void* partial, void* const* h
                                              void* mc_ag_recv, int rank, int nranks, int slot, void* epoch_state, void* x_out,
                                              void* residual, const void* weight, float eps, int64_t num_tokens, int hidden,
                                              int64_t rows_per_rank, sllm_dtype_t dtype, sllm_stream_t stream) {
-    SLLM_REQUIRE(nranks >= 2 && nranks <= LL_MAX_RANKS && rank >= 0 && rank < nranks, "allreduce(LL): bad rank %d of %d", rank, nranks);
-    SLLM_REQUIRE(slot >= 0 && slot < 16, "allreduce(LL): bad slot %d", slot);
-    SLLM_REQUIRE(hidden > 0 && hidden % 8 == 0 && num_tokens >= 0, "allreduce(LL): hidden (%d) must be a positive multiple of 8", hidden);
+    if (check_exchange("allreduce(LL)", rank, nranks, slot, 16, hidden, num_tokens)) return 1;
     if (num_tokens == 0) return 0;
     SLLM_REQUIRE(rows_per_rank > 0 && num_tokens <= rows_per_rank * nranks,
                  "allreduce(LL): %lld tokens exceed the receive buffers (%lld rows per rank x %d ranks)", (long long)num_tokens,
@@ -219,30 +186,12 @@ extern "C" int sllm_allreduce_add_rmsnorm_ll(const void* partial, void* const* h
     p.partial = partial; p.mc_ag_recv = mc_ag_recv; p.x_out = x_out; p.residual = residual; p.weight = weight;
     p.epoch = (uint32_t*)epoch_state; p.eps = eps; p.rank = rank; p.nranks = nranks; p.hidden = hidden; p.slot = slot;
     p.num_tokens = (int)num_tokens; p.rows_per_rank = (int)rows_per_rank;
-    const int nvec = hidden / 8;
-    int threads = nvec >= 512 ? 512 : (nvec >= 256 ? 256 : ((nvec + 31) / 32) * 32);
-    if (threads < 32) threads = 32;
-    const size_t smem = (size_t)nvec * sizeof(uint4);
-    SLLM_REQUIRE(smem <= 48 * 1024, "allreduce(LL): hidden %d too large", hidden);
-    static int sm_count[64] = {0};                                   // per device (a process may drive several)
-    const int dev = current_device() & 63;
-    if (sm_count[dev] == 0) {
-        int n = 0;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sm_count[dev] = n > 0 ? n : 132;
-    }
-    const int64_t cap = 2LL * sm_count[dev];                         // one wave below 512 threads, two at 512: see the kernel comment
+    SLLM_REQUIRE((size_t)(hidden / 8) * sizeof(uint4) <= 48 * 1024, "allreduce(LL): hidden %d too large", hidden);
+    const int64_t cap = 2LL * num_sms();                             // one wave below 512 threads, two at 512: see the kernel comment
     const unsigned grid = (unsigned)(num_tokens < cap ? num_tokens : cap);
-    cudaStream_t st = (cudaStream_t)stream;
     const bool nvls = mc_ag_recv != nullptr;
-    if (dtype == SLLM_F16) {
-        if (nvls) allreduce_add_rmsnorm_ll_kernel<__half, true><<<grid, threads, smem, st>>>(p);
-        else allreduce_add_rmsnorm_ll_kernel<__half, false><<<grid, threads, smem, st>>>(p);
-    } else if (dtype == SLLM_BF16) {
-        if (nvls) allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, true><<<grid, threads, smem, st>>>(p);
-        else allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, false><<<grid, threads, smem, st>>>(p);
-    } else {
-        SLLM_REQUIRE(false, "allreduce(LL): unknown dtype tag %d", (int)dtype);
-    }
-    return check_launch("allreduce_add_rmsnorm_ll");
+    return launch_exchange("allreduce(LL)", "allreduce_add_rmsnorm_ll",
+                           nvls ? allreduce_add_rmsnorm_ll_kernel<__half, true> : allreduce_add_rmsnorm_ll_kernel<__half, false>,
+                           nvls ? allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, true> : allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, false>,
+                           dtype, grid, hidden, (cudaStream_t)stream, p);
 }

@@ -11,59 +11,33 @@
 // consecutive exchanges, so a rank can only overwrite a buffer after every peer has passed the barrier of the
 // exchange in between, i.e. finished reading it.  Epochs live in device memory (CUDA-graph replay safe).
 // A watchdog traps instead of hanging if a peer never arrives.
-#include <type_traits>
-
-#include "common.cuh"
+// Flags, peer loads, the rank-ordered sum, the epoch step and the host checks / launch are shared with allreduce_ll.cu
+// (exchange.cuh); the add + RMSNorm row epilogue with rmsnorm_kernel (common.cuh).
+#include "exchange.cuh"
 
 namespace sllm {
 
-constexpr int AR_MAX_RANKS = 8;
-
 struct ArParams {
-    const void* peer_buf[AR_MAX_RANKS];      // partial [T, H] of every rank (peer-mapped device pointers)
-    uint32_t* peer_flags[AR_MAX_RANKS];      // signal pad of every rank: uint32 [slots][AR_MAX_RANKS]
+    const void* peer_buf[MAX_RANKS];         // partial [T, H] of every rank (peer-mapped device pointers)
+    uint32_t* peer_flags[MAX_RANKS];         // signal pad of every rank: uint32 [slots][MAX_RANKS]
     uint32_t* epoch;                         // local device memory: uint32 [slots] epoch, then uint32 [slots] done-counter
     void* x_out; void* residual; const void* weight;
     float eps;
     int rank, nranks, hidden, slot, has_norm;
 };
 
-__device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-
-// peer data is produced by another GPU while this kernel may already be running: no read-only / L1 caching
-template <typename T> __device__ __forceinline__ Vec8<T> ld_vec8_peer(const T* p) {
-    uint4 u;
-    asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(p) : "memory");
-    return *reinterpret_cast<Vec8<T>*>(&u);
-}
-
 template <typename T>
 __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_kernel(const ArParams p) {
     extern __shared__ uint4 row_smem[];
     __shared__ float red[16];
-    using TT = Traits<T>;
     const int64_t t = blockIdx.x;
     const int nvec = p.hidden >> 3;
     const uint32_t e = p.epoch[p.slot] + 1;                 // epoch of this exchange (same value in every CTA)
 
     // ---- barrier: my partial is complete (stream order) -> tell every peer; wait for every peer's flag
     if (threadIdx.x < p.nranks) {
-        if (blockIdx.x == 0) {
-            __threadfence_system();
-            st_release_sys(p.peer_flags[threadIdx.x] + p.slot * AR_MAX_RANKS + p.rank, e);
-        }
-        const uint32_t* mine = p.peer_flags[p.rank] + p.slot * AR_MAX_RANKS + threadIdx.x;
-        uint32_t spins = 0;
-        while ((int32_t)(ld_acquire_sys(mine) - e) < 0) {
-            if (++spins > (1u << 27)) { printf("sllm: all-reduce watchdog (rank %d waits for rank %d, epoch %u)\n", p.rank, threadIdx.x, e); __trap(); }
-        }
+        if (blockIdx.x == 0) publish_flag(p, 0, e);
+        wait_flag(p, 0, e, "sllm: all-reduce watchdog (rank %d waits for rank %d, epoch %u)\n");
     }
     __syncthreads();
 
@@ -71,57 +45,22 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_kernel(const ArPara
     T* rr = reinterpret_cast<T*>(p.residual) + t * p.hidden;
     float ss = 0.f;
     for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        // all N peer loads are issued before the first one is consumed (one NVLink round trip instead of N in series);
-        // the accumulation below keeps the fixed rank order -> identical sums on every rank
-        Vec8<T> pv[AR_MAX_RANKS];
-#pragma unroll
-        for (int r = 0; r < AR_MAX_RANKS; r++)
-            if (r < p.nranks) pv[r] = ld_vec8_peer(reinterpret_cast<const T*>(p.peer_buf[r]) + t * p.hidden + 8 * i);
-#pragma unroll
-        for (int r = 0; r < AR_MAX_RANKS; r++) {
-            if (r < p.nranks) {
-#pragma unroll
-                for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(pv[r].v[j]); acc[2 * j] += f.x; acc[2 * j + 1] += f.y; }
-            }
-        }
-        Vec8<T> a, b = ld_vec8(rr + 8 * i);
-#pragma unroll
-        for (int j = 0; j < 4; j++) a.v[j] = __hadd2_rn(TT::from_f2(make_float2(acc[2 * j], acc[2 * j + 1])), b.v[j]);   // h(h(sum) + r)
-        st_vec8(rr + 8 * i, a);
-        row_smem[i] = *reinterpret_cast<uint4*>(&a);
-#pragma unroll
-        for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(a.v[j]); ss += f.x * f.x + f.y * f.y; }
+        Vec8<T> sum;
+        peer_sum(sum, p.peer_buf, p.nranks, t * p.hidden + 8 * i);
+        add_residual(sum, rr + 8 * i, &row_smem[i], ss);
     }
     if (p.has_norm) {
-        ss = warp_sum(ss);
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-        if (lane == 0) red[warp] = ss;
-        __syncthreads();
-        float total = 0.f;
-        for (int w = 0; w < nwarps; w++) total += red[w];
-        const float rstd = 1.0f / sqrtf(total / (float)p.hidden + p.eps);
+        const float rstd = row_rstd(warp_sum(ss), red, p.hidden, p.eps);
         T* xo = reinterpret_cast<T*>(p.x_out) + t * p.hidden;
         const T* wt = reinterpret_cast<const T*>(p.weight);
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-            Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
-            Vec8<T> w = ld_vec8(wt + 8 * i);
+            const Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
             Vec8<T> o;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                float2 f = TT::to_f2(a.v[j]), g = TT::to_f2(w.v[j]);
-                o.v[j] = TT::from_f2(make_float2((f.x * rstd) * g.x, (f.y * rstd) * g.y));
-            }
+            rms_scale(o, a, rstd, wt + 8 * i);
             st_vec8(xo + 8 * i, o);
         }
     }
-
-    // ---- the last CTA to finish advances the epoch (all CTAs have read it by then)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t* done = p.epoch + 16 + p.slot;
-        if (atomicAdd(done, 1u) == gridDim.x - 1) { *done = 0; __threadfence(); p.epoch[p.slot] = e; }
-    }
+    advance_epoch(p.epoch, p.slot, e);
 }
 
 // ------------------------------------------------------------------ two-shot variant (reduce-scatter + all-gather by token rows)
@@ -138,9 +77,9 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_kernel(const ArPara
 // A single x_out buffer per rank suffices: a peer can only write exchange k+1's rows after barrier A of k+1, i.e. after this
 // rank has launched k+1, which is after everything that consumed x_out of exchange k in its stream.
 struct Ar2Params {
-    const void* peer_buf[AR_MAX_RANKS];      // partial [T, H] of every rank
-    void* peer_xout[AR_MAX_RANKS];           // x_out [T, H] of every rank (symmetric, written by the row owners)
-    uint32_t* peer_flags[AR_MAX_RANKS];      // signal pad of every rank: uint32 [16][AR_MAX_RANKS]; rows slot (A) and 8 + slot (B)
+    const void* peer_buf[MAX_RANKS];         // partial [T, H] of every rank
+    void* peer_xout[MAX_RANKS];              // x_out [T, H] of every rank (symmetric, written by the row owners)
+    uint32_t* peer_flags[MAX_RANKS];         // signal pad of every rank: uint32 [16][MAX_RANKS]; rows slot (A) and 8 + slot (B)
     uint32_t* epoch;
     void* residual; const void* weight;
     float eps;
@@ -165,14 +104,6 @@ template <> __device__ __forceinline__ Vec8<__nv_bfloat16> multimem_ld_reduce_ad
                  : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(mc) : "memory");
     return *reinterpret_cast<Vec8<__nv_bfloat16>*>(&u);
 }
-template <typename T> __device__ __forceinline__ void multimem_st(T* mc, const Vec8<T>& v) {
-    const uint4 u = *reinterpret_cast<const uint4*>(&v);
-    if constexpr (sizeof(T) == 2 && std::is_same<T, __half>::value)
-        asm volatile("multimem.st.relaxed.sys.global.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(mc), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
-    else
-        asm volatile("multimem.st.relaxed.sys.global.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(mc), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
-}
-
 template <typename T> __device__ __forceinline__ void st_vec8_peer(T* p, const Vec8<T>& v) {
     const uint4 u = *reinterpret_cast<const uint4*>(&v);
     asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
@@ -183,7 +114,6 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_2shot_kernel(const 
     extern __shared__ uint4 row_smem[];
     __shared__ float red[16];
     __shared__ int s_last;
-    using TT = Traits<T>;
     const int64_t t = (int64_t)blockIdx.x * p.nranks + p.rank;     // the row this CTA owns (may be past the end)
     const int nvec = p.hidden >> 3;
     const uint32_t e = p.epoch[p.slot] + 1;
@@ -191,13 +121,8 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_2shot_kernel(const 
     // ---- barrier A.  EVERY CTA publishes (idempotent: the same epoch value; the partial is complete for all of them by stream
     // order), so progress never depends on CTA 0 being dispatched before the CTAs that wait.
     if (threadIdx.x < p.nranks) {
-        __threadfence_system();
-        st_release_sys(p.peer_flags[threadIdx.x] + p.slot * AR_MAX_RANKS + p.rank, e);
-        const uint32_t* mine = p.peer_flags[p.rank] + p.slot * AR_MAX_RANKS + threadIdx.x;
-        uint32_t spins = 0;
-        while ((int32_t)(ld_acquire_sys(mine) - e) < 0) {
-            if (++spins > (1u << 27)) { printf("sllm: two-shot all-reduce watchdog A (rank %d waits for rank %d, epoch %u)\n", p.rank, threadIdx.x, e); __trap(); }
-        }
+        publish_flag(p, 0, e);
+        wait_flag(p, 0, e, "sllm: two-shot all-reduce watchdog A (rank %d waits for rank %d, epoch %u)\n");
     }
     __syncthreads();
 
@@ -207,56 +132,24 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_2shot_kernel(const 
         float ss = 0.f;
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
             Vec8<T> sum;                                            // h(sum over ranks)
-            if constexpr (NVLS) {
-                sum = multimem_ld_reduce_add<T>(reinterpret_cast<const T*>(p.mc_buf) + t * p.hidden + 8 * i);
-            } else {
-                float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                Vec8<T> pv[AR_MAX_RANKS];                           // N independent peer loads in flight, summed in rank order
-#pragma unroll
-                for (int r = 0; r < AR_MAX_RANKS; r++)
-                    if (r < p.nranks) pv[r] = ld_vec8_peer(reinterpret_cast<const T*>(p.peer_buf[r]) + t * p.hidden + 8 * i);
-#pragma unroll
-                for (int r = 0; r < AR_MAX_RANKS; r++) {
-                    if (r < p.nranks) {
-#pragma unroll
-                        for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(pv[r].v[j]); acc[2 * j] += f.x; acc[2 * j + 1] += f.y; }
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < 4; j++) sum.v[j] = TT::from_f2(make_float2(acc[2 * j], acc[2 * j + 1]));
-            }
-            Vec8<T> a, b = ld_vec8(rr + 8 * i);
-#pragma unroll
-            for (int j = 0; j < 4; j++) a.v[j] = __hadd2_rn(sum.v[j], b.v[j]);   // h(h(sum) + r)
-            st_vec8(rr + 8 * i, a);
-            row_smem[i] = *reinterpret_cast<uint4*>(&a);
-#pragma unroll
-            for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(a.v[j]); ss += f.x * f.x + f.y * f.y; }
+            if constexpr (NVLS) sum = multimem_ld_reduce_add<T>(reinterpret_cast<const T*>(p.mc_buf) + t * p.hidden + 8 * i);
+            else peer_sum(sum, p.peer_buf, p.nranks, t * p.hidden + 8 * i);
+            add_residual(sum, rr + 8 * i, &row_smem[i], ss);
         }
-        ss = warp_sum(ss);
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-        if (lane == 0) red[warp] = ss;
-        __syncthreads();
-        float total = 0.f;
-        for (int w = 0; w < nwarps; w++) total += red[w];
-        const float rstd = 1.0f / sqrtf(total / (float)p.hidden + p.eps);
+        const float rstd = row_rstd(warp_sum(ss), red, p.hidden, p.eps);
         const T* wt = reinterpret_cast<const T*>(p.weight);
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-            Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
-            Vec8<T> w = ld_vec8(wt + 8 * i);
+            const Vec8<T> a = *reinterpret_cast<Vec8<T>*>(&row_smem[i]);
             Vec8<T> o;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                float2 f = TT::to_f2(a.v[j]), g = TT::to_f2(w.v[j]);
-                o.v[j] = TT::from_f2(make_float2((f.x * rstd) * g.x, (f.y * rstd) * g.y));
-            }
+            rms_scale(o, a, rstd, wt + 8 * i);
             // ---- all-gather: the normalised row goes to every rank (own copy included), starting with the next rank so the
             // N owners do not all hit the same destination at the same time
             if constexpr (NVLS) {
-                multimem_st<T>(reinterpret_cast<T*>(p.mc_xout) + t * p.hidden + 8 * i, o);
+                const uint4 u = *reinterpret_cast<const uint4*>(&o);
+                multimem_st(reinterpret_cast<T*>(p.mc_xout) + t * p.hidden + 8 * i, u.x, u.y, u.z, u.w);
             } else {
 #pragma unroll
-                for (int k = 0; k < AR_MAX_RANKS; k++) {
+                for (int k = 0; k < MAX_RANKS; k++) {
                     if (k < p.nranks) {
                         int r = p.rank + 1 + k;
                         if (r >= p.nranks) r -= p.nranks;
@@ -278,13 +171,8 @@ __global__ void __launch_bounds__(512) allreduce_add_rmsnorm_2shot_kernel(const 
     __syncthreads();
     if (!s_last) return;
     if (threadIdx.x < p.nranks) {
-        __threadfence_system();
-        st_release_sys(p.peer_flags[threadIdx.x] + (8 + p.slot) * AR_MAX_RANKS + p.rank, e);
-        const uint32_t* mine = p.peer_flags[p.rank] + (8 + p.slot) * AR_MAX_RANKS + threadIdx.x;
-        uint32_t spins = 0;
-        while ((int32_t)(ld_acquire_sys(mine) - e) < 0) {
-            if (++spins > (1u << 27)) { printf("sllm: two-shot all-reduce watchdog B (rank %d waits for rank %d, epoch %u)\n", p.rank, threadIdx.x, e); __trap(); }
-        }
+        publish_flag(p, 8, e);
+        wait_flag(p, 8, e, "sllm: two-shot all-reduce watchdog B (rank %d waits for rank %d, epoch %u)\n");
     }
     __syncthreads();
     if (threadIdx.x == 0) { __threadfence(); p.epoch[p.slot] = e; }     // every CTA of this launch has read the epoch by now
@@ -304,10 +192,7 @@ extern "C" int sllm_allreduce_add_rmsnorm_2shot(const void* const* host_peer_buf
                                                 float eps, int64_t num_tokens, int hidden, sllm_dtype_t dtype,
                                                 sllm_stream_t stream) {
     SLLM_REQUIRE((mc_buf == nullptr) == (mc_xout == nullptr), "allreduce(2-shot): give both multicast addresses or neither");
-    SLLM_REQUIRE(nranks >= 2 && nranks <= AR_MAX_RANKS && rank >= 0 && rank < nranks, "allreduce(2-shot): bad rank %d of %d", rank, nranks);
-    SLLM_REQUIRE(slot >= 0 && slot < 8, "allreduce(2-shot): bad slot %d", slot);
-    SLLM_REQUIRE(hidden > 0 && hidden % 8 == 0 && num_tokens >= 0 && num_tokens < (1LL << 31),
-                 "allreduce(2-shot): hidden (%d) must be a positive multiple of 8", hidden);
+    if (check_exchange("allreduce(2-shot)", rank, nranks, slot, 8, hidden, num_tokens)) return 1;
     if (num_tokens == 0) return 0;
     SLLM_REQUIRE(host_peer_bufs && host_peer_xout && host_peer_flags && epoch_state && residual && weight, "allreduce(2-shot): null pointer");
     Ar2Params p;
@@ -318,26 +203,11 @@ extern "C" int sllm_allreduce_add_rmsnorm_2shot(const void* const* host_peer_buf
     p.rank = rank; p.nranks = nranks; p.hidden = hidden; p.slot = slot; p.num_tokens = (int)num_tokens;
     p.mc_buf = mc_buf; p.mc_xout = mc_xout;
     const bool nvls = mc_buf != nullptr;
-    const int nvec = hidden / 8;
-    int threads = nvec >= 512 ? 512 : (nvec >= 256 ? 256 : ((nvec + 31) / 32) * 32);
-    if (threads < 32) threads = 32;
-    const size_t smem = (size_t)nvec * sizeof(uint4);
     const unsigned grid = (unsigned)((num_tokens + nranks - 1) / nranks);        // the same on every rank
-    cudaStream_t st = (cudaStream_t)stream;
-#define SLLM_AR2_LAUNCH(TT, NV)                                                                                                   \
-    do {                                                                                                                          \
-        if (smem > 48 * 1024) cudaFuncSetAttribute(allreduce_add_rmsnorm_2shot_kernel<TT, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        allreduce_add_rmsnorm_2shot_kernel<TT, NV><<<grid, threads, smem, st>>>(p);                                               \
-    } while (0)
-    if (dtype == SLLM_F16) {
-        if (nvls) SLLM_AR2_LAUNCH(__half, true); else SLLM_AR2_LAUNCH(__half, false);
-    } else if (dtype == SLLM_BF16) {
-        if (nvls) SLLM_AR2_LAUNCH(__nv_bfloat16, true); else SLLM_AR2_LAUNCH(__nv_bfloat16, false);
-    } else {
-        SLLM_REQUIRE(false, "allreduce(2-shot): unknown dtype tag %d", (int)dtype);
-    }
-#undef SLLM_AR2_LAUNCH
-    return check_launch("allreduce_add_rmsnorm_2shot");
+    return launch_exchange("allreduce(2-shot)", "allreduce_add_rmsnorm_2shot",
+                           nvls ? allreduce_add_rmsnorm_2shot_kernel<__half, true> : allreduce_add_rmsnorm_2shot_kernel<__half, false>,
+                           nvls ? allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, true> : allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, false>,
+                           dtype, grid, hidden, (cudaStream_t)stream, p);
 }
 
 // host_peer_bufs / host_peer_flags: HOST arrays of `nranks` device pointers (the symmetric buffer and the signal pad of
@@ -346,28 +216,13 @@ extern "C" int sllm_allreduce_add_rmsnorm_2shot(const void* const* host_peer_buf
 extern "C" int sllm_allreduce_add_rmsnorm(const void* const* host_peer_bufs, void* const* host_peer_flags, int rank, int nranks,
                                           int slot, void* epoch_state, void* x_out, void* residual, const void* weight, float eps,
                                           int64_t num_tokens, int hidden, sllm_dtype_t dtype, sllm_stream_t stream) {
-    SLLM_REQUIRE(nranks >= 2 && nranks <= AR_MAX_RANKS && rank >= 0 && rank < nranks, "allreduce: bad rank %d of %d", rank, nranks);
-    SLLM_REQUIRE(slot >= 0 && slot < 16, "allreduce: bad slot %d", slot);
-    SLLM_REQUIRE(hidden > 0 && hidden % 8 == 0 && num_tokens >= 0, "allreduce: hidden (%d) must be a positive multiple of 8", hidden);
+    if (check_exchange("allreduce", rank, nranks, slot, 16, hidden, num_tokens)) return 1;
     if (num_tokens == 0) return 0;
     SLLM_REQUIRE(host_peer_bufs && host_peer_flags && epoch_state && residual && (weight == nullptr || x_out), "allreduce: null pointer");
     ArParams p;
     for (int r = 0; r < nranks; r++) { p.peer_buf[r] = host_peer_bufs[r]; p.peer_flags[r] = (uint32_t*)host_peer_flags[r]; }
     p.epoch = (uint32_t*)epoch_state; p.x_out = x_out; p.residual = residual; p.weight = weight; p.eps = eps;
     p.rank = rank; p.nranks = nranks; p.hidden = hidden; p.slot = slot; p.has_norm = weight != nullptr;
-    const int nvec = hidden / 8;
-    int threads = nvec >= 512 ? 512 : (nvec >= 256 ? 256 : ((nvec + 31) / 32) * 32);
-    if (threads < 32) threads = 32;
-    const size_t smem = (size_t)nvec * sizeof(uint4);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == SLLM_F16) {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(allreduce_add_rmsnorm_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        allreduce_add_rmsnorm_kernel<__half><<<(unsigned)num_tokens, threads, smem, st>>>(p);
-    } else if (dtype == SLLM_BF16) {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(allreduce_add_rmsnorm_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        allreduce_add_rmsnorm_kernel<__nv_bfloat16><<<(unsigned)num_tokens, threads, smem, st>>>(p);
-    } else {
-        SLLM_REQUIRE(false, "allreduce: unknown dtype tag %d", (int)dtype);
-    }
-    return check_launch("allreduce_add_rmsnorm");
+    return launch_exchange("allreduce", "allreduce_add_rmsnorm", allreduce_add_rmsnorm_kernel<__half>,
+                           allreduce_add_rmsnorm_kernel<__nv_bfloat16>, dtype, (unsigned)num_tokens, hidden, (cudaStream_t)stream, p);
 }

@@ -79,6 +79,51 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+// ---------------------------------------------------------------- add + RMSNorm row epilogue
+// One CTA per token row of `nvec` 16-byte vectors (row_threads threads), the rounding order of rmsnorm.py:39-65.  rmsnorm_kernel
+// and the three exchange kernels build their rows from these, which is what keeps x_out bit-identical across them.
+
+template <typename T> __device__ __forceinline__ void add_sum_sq(float& ss, const Vec8<T>& a) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) { float2 f = Traits<T>::to_f2(a.v[j]); ss += f.x * f.x + f.y * f.y; }
+}
+// a = h(sum + r) for one vector: stored back to the residual at rr, stashed for the normalise pass, added to the sum of squares
+template <typename T> __device__ __forceinline__ void add_residual(const Vec8<T>& sum, T* rr, uint4* stash, float& ss) {
+    Vec8<T> a, b = ld_vec8(rr);
+#pragma unroll
+    for (int j = 0; j < 4; j++) a.v[j] = __hadd2_rn(sum.v[j], b.v[j]);
+    st_vec8(rr, a);
+    *stash = *reinterpret_cast<uint4*>(&a);
+    add_sum_sq(ss, a);
+}
+// 1 / rms of the row from every thread's warp_sum of its sum of squares.  red[] holds one float per warp; every thread adds it in
+// the same order -> identical rstd.  A caller that reuses red[] for another row synchronises before calling again.  hidden and eps
+// by reference: an exchange kernel then reads them from its parameter struct after the barrier, which keeps its schedule.
+__device__ __forceinline__ float row_rstd(float warp_ss, float* red, const int& hidden, const float& eps) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    if (lane == 0) red[warp] = warp_ss;
+    __syncthreads();
+    float total = 0.f;
+    for (int w = 0; w < nwarps; w++) total += red[w];
+    return 1.0f / sqrtf(total / (float)hidden + eps);
+}
+// o = (a * rstd) * w, one rounding.  `a` may live in shared memory (read after w is loaded); o is an out-parameter because a
+// returned Vec8 compiles rmsnorm_kernel to a different schedule.
+template <typename T> __device__ __forceinline__ void rms_scale(Vec8<T>& o, const Vec8<T>& a, float rstd, const T* w) {
+    using TT = Traits<T>;
+    Vec8<T> g8 = ld_vec8(w);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        float2 f = TT::to_f2(a.v[j]), g = TT::to_f2(g8.v[j]);
+        o.v[j] = TT::from_f2(make_float2((f.x * rstd) * g.x, (f.y * rstd) * g.y));
+    }
+}
+// threads per row of nvec vectors: one vector per thread up to 512, whole warps
+static inline int row_threads(int nvec) {
+    const int threads = nvec >= 512 ? 512 : (nvec >= 256 ? 256 : ((nvec + 31) / 32) * 32);
+    return threads < 32 ? 32 : threads;
+}
+
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 // ---------------------------------------------------------------- per-device one-time state (a process may drive several GPUs)
@@ -87,6 +132,7 @@ static inline int current_device() {
     cudaGetDevice(&d);
     return d;
 }
+int num_sms();   // multiprocessors of the current device, cached
 // true exactly once per (call site's mask, device): e.g. cudaFuncSetAttribute, which is a per-device setting
 static inline bool first_use_on_this_device(unsigned long long& mask) {
     const unsigned long long bit = 1ull << (current_device() & 63);

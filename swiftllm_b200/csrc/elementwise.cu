@@ -3,7 +3,7 @@
 // order of the reference Triton kernels (SURVEY.md Appendix A; oracle/kernels.py restates them):
 //   rmsnorm.py:5-24, :39-65   rotary_emb.py:7-41   silu_and_mul.py:5-23
 // Algorithmic bytes (s = 2): rmsnorm 2*T*H*s + H*s, fused 4*T*H*s + H*s, rotary 2*T*(nq+nkv)*D*s + T*D*s,
-// silu_and_mul 3*T*F*s.
+// silu_and_mul 3*T*F*s.  The RMSNorm row epilogue (add_residual / row_rstd / rms_scale, common.cuh) is the exchange kernels' too.
 #include "common.cuh"
 
 namespace sllm {
@@ -18,7 +18,6 @@ __global__ void __launch_bounds__(512) rmsnorm_kernel(T* __restrict__ x, T* __re
                                                       const T* __restrict__ weight, float eps, int hidden) {
     extern __shared__ uint4 row_smem[];
     __shared__ float red[16];
-    using TT = Traits<T>;
     const int64_t t = blockIdx.x;
     T* xr = x + t * hidden;
     T* rr = FUSED_ADD ? residual + t * hidden : nullptr;
@@ -42,47 +41,34 @@ __global__ void __launch_bounds__(512) rmsnorm_kernel(T* __restrict__ x, T* __re
                 for (int j = 0; j < 4; j++) regs[v].v[j] = __hadd2_rn(regs[v].v[j], rv[v].v[j]);   // s = h(x + r): storage-dtype add
                 st_vec8(rr + 8 * (threadIdx.x + v * blockDim.x), regs[v]);
             }
-#pragma unroll
-            for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(regs[v].v[j]); ss += f.x * f.x + f.y * f.y; }
+            add_sum_sq(ss, regs[v]);
         }
     } else {
         for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
             Vec8<T> a = ld_vec8(xr + 8 * i);
             if (FUSED_ADD) {
-                Vec8<T> b = ld_vec8(rr + 8 * i);
-#pragma unroll
-                for (int j = 0; j < 4; j++) a.v[j] = __hadd2_rn(a.v[j], b.v[j]);
-                st_vec8(rr + 8 * i, a);
+                add_residual(a, rr + 8 * i, &row_smem[i], ss);
+            } else {
+                row_smem[i] = *reinterpret_cast<uint4*>(&a);
+                add_sum_sq(ss, a);
             }
-            row_smem[i] = *reinterpret_cast<uint4*>(&a);
-#pragma unroll
-            for (int j = 0; j < 4; j++) { float2 f = TT::to_f2(a.v[j]); ss += f.x * f.x + f.y * f.y; }
         }
     }
-    ss = warp_sum(ss);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    if (lane == 0) red[warp] = ss;
-    __syncthreads();
-    float total = 0.f;
-    for (int w = 0; w < nwarps; w++) total += red[w];      // same order in every thread -> identical rstd
-    const float rstd = 1.0f / sqrtf(total / (float)hidden + eps);
-
-    auto finish = [&](const Vec8<T>& a, int i) {
-        Vec8<T> w = ld_vec8(weight + 8 * i);
-        Vec8<T> o;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            float2 f = TT::to_f2(a.v[j]);
-            float2 g = TT::to_f2(w.v[j]);
-            o.v[j] = TT::from_f2(make_float2((f.x * rstd) * g.x, (f.y * rstd) * g.y));
-        }
-        st_vec8(xr + 8 * i, o);
-    };
+    const float rstd = row_rstd(warp_sum(ss), red, hidden, eps);
     if (VPT > 0) {
 #pragma unroll
-        for (int v = 0; v < NV; v++) finish(regs[v], threadIdx.x + v * blockDim.x);
+        for (int v = 0; v < NV; v++) {
+            const int i = threadIdx.x + v * blockDim.x;
+            Vec8<T> o;
+            rms_scale(o, regs[v], rstd, weight + 8 * i);
+            st_vec8(xr + 8 * i, o);
+        }
     } else {
-        for (int i = threadIdx.x; i < nvec; i += blockDim.x) finish(*reinterpret_cast<Vec8<T>*>(&row_smem[i]), i);
+        for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+            Vec8<T> o;
+            rms_scale(o, *reinterpret_cast<Vec8<T>*>(&row_smem[i]), rstd, weight + 8 * i);
+            st_vec8(xr + 8 * i, o);
+        }
     }
 }
 
@@ -101,8 +87,7 @@ static int launch_rmsnorm(void* x, void* residual, const void* weight, float eps
         rmsnorm_kernel<T, FUSED, 2><<<(unsigned)T_, nvec / 2, 0, stream>>>((T*)x, (T*)residual, (const T*)weight, eps, hidden);
         return check_launch(what);
     }
-    int threads = nvec >= 512 ? 512 : (nvec >= 256 ? 256 : ((nvec + 31) / 32) * 32);
-    if (threads < 32) threads = 32;
+    const int threads = row_threads(nvec);
     size_t smem = (size_t)nvec * sizeof(uint4);
     if (smem > 48 * 1024)
         cudaFuncSetAttribute(rmsnorm_kernel<T, FUSED, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -35,6 +35,17 @@ int forced_generation(const char* env_var) {
     return (e && e[0] == '1') ? 1 : (e && e[0] == '2') ? 2 : 0;
 }
 
+int num_sms() {
+    static int sms[64] = {0};
+    const int dev = current_device() & 63;
+    if (sms[dev] == 0) {
+        int n = 0;
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        sms[dev] = n > 0 ? n : 132;
+    }
+    return sms[dev];
+}
+
 namespace tc {
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 TensorMapEncodeFn get_tensor_map_encoder() {

@@ -260,17 +260,6 @@ static int64_t partial_bytes(int64_t rows, int nq, int64_t num_splits, int head_
 }
 
 // ---- host-side split policy (v1 vs v2)
-static int num_sms() {                       // of the CURRENT device (a process may drive several)
-    static int sms[64] = {0};
-    const int dev = current_device() & 63;
-    if (sms[dev] == 0) {
-        int n = 0;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms[dev] = n > 0 ? n : 132;
-    }
-    return sms[dev];
-}
-
 // Tokens per flash-decoding split (a multiple of 128), shared by both kernel generations so the workspace size
 // does not depend on which one runs.  Fixed by the caller when seq_block_size > 0.
 static int choose_split_tokens(int num_seqs, int nkv, int max_seq_len, int seq_block_size) {
