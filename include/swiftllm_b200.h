@@ -331,6 +331,22 @@ int sllm_apply_penalties(void* logits, int64_t num_rows, int vocab_size, int64_t
                          const int32_t* block_table, int block_table_stride, int block_size, int32_t* token_cache,
                          int64_t num_blocks, sllm_dtype_t dtype, sllm_stream_t stream);
 
+/* ---- Constrained decoding (new): allowed-token bitmasks and logit bias, IN PLACE on logits laid out as in sllm_sample_tokens
+ * (a vocabulary shard with vocab_offset works; bits and bias ids are global indices).  Per-row DEVICE arrays [num_rows]:
+ * mask_index (-1: no mask; else a row of masks uint32 [num_masks, mask_words], bit v % 32 of word v / 32 set = id v allowed)
+ * and bias_index (-1: no bias; else an entry e of the CSR arrays bias_starts int32 [num_entries + 1], bias_ids int32 [num_bias]
+ * (distinct within an entry) and bias_values fp32 [num_bias]).  Every disallowed id becomes -inf; then every allowed id with a
+ * bias becomes round(float(l) + b), one fp32 add and one rounding to the storage dtype.  Rows with neither are not touched;
+ * allowed unbiased entries keep their bits.  Out-of-range mask / bias indices and bias ids outside the shard are skipped.
+ * Deterministic: each logit is written by at most one thread.  Rejected before launch: unknown dtype, vocab_size <= 0, global
+ * indices >= 2^31, a row stride below vocab_size, mask_words that do not cover vocab_offset + vocab_size ids (when num_masks >
+ * 0), negative or too large counts, null pointers (masks / bias_starts / bias_ids and bias_values may be NULL when their count
+ * is 0).  num_rows == 0 is a no-op. */
+int sllm_constrain_logits(void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride, int64_t vocab_offset,
+                          const int32_t* mask_index, const uint32_t* masks, int64_t num_masks, int mask_words,
+                          const int32_t* bias_index, const int32_t* bias_starts, int64_t num_entries, const int32_t* bias_ids,
+                          const float* bias_values, int64_t num_bias, sllm_dtype_t dtype, sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

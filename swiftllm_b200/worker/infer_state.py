@@ -60,6 +60,9 @@ class LlamaInferState:
     # Prompt log-probabilities (SamplingParams.prompt_logprobs): the prefill rows to score; None = none, and the post layer
     # returns what it returned before
     prompt_logprobs: Optional["PromptLogprobsState"] = None
+    # Allowed-token masks and logit bias of the step's last rows (csrc/constraints.cu); None = no row is constrained.  Kept apart
+    # from `sampling`: a constrained step may be greedy with no sampling parameters at all
+    constraints: Optional["ConstraintState"] = None
 
 
 @dataclasses.dataclass
@@ -111,3 +114,24 @@ class SamplingState:
         return SamplingState(temperature=words[2 * B:3 * B].view(torch.float32), top_k=words[3 * B:4 * B],
                              top_p=words[4 * B:5 * B].view(torch.float32), seed=words[:2 * B].view(torch.int64), pos=pos,
                              filtered=filtered, sampled=sampled, **pen)
+
+
+@dataclasses.dataclass
+class ConstraintState:
+    """Device views of the staged constraint region (swiftllm_b200.sampling_params.constraint_words), one row per last row."""
+    mask_index: torch.Tensor        # [rows] int32: row of `masks`, -1 = no mask
+    masks: torch.Tensor             # [num_masks, W] int32 bit words of global ids
+    bias_index: torch.Tensor        # [rows] int32: bias entry, -1 = no bias
+    bias_starts: torch.Tensor       # [num_entries + 1] int32 CSR starts
+    bias_ids: torch.Tensor          # [num_bias] int32 global ids (-1: padding, matches no id)
+    bias_values: torch.Tensor       # [num_bias] float32
+
+    @staticmethod
+    def from_staged(words: torch.Tensor, num_rows: int, num_masks: int, mask_words: int, num_entries: int,
+                    num_bias: int) -> "ConstraintState":
+        R, E, NB = num_rows, num_entries, num_bias
+        o = [0, R, 2 * R, 2 * R + E + 1, 2 * R + E + 1 + NB, 2 * R + E + 1 + 2 * NB]
+        assert words.shape[0] == o[5] + num_masks * mask_words
+        return ConstraintState(mask_index=words[:o[1]], bias_index=words[o[1]:o[2]], bias_starts=words[o[2]:o[3]],
+                               bias_ids=words[o[3]:o[4]], bias_values=words[o[4]:o[5]].view(torch.float32),
+                               masks=words[o[5]:].view(num_masks, mask_words))

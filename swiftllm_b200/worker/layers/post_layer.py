@@ -23,11 +23,18 @@ the same tokens in its own pages.
 Addition (prompt log-probabilities, csrc/prompt_logprobs.cu): when the step scores prompt rows (infer_state.prompt_logprobs),
 the last-row path above runs first, unchanged; then the prompt rows go through the final RMSNorm, lm_head (gathered when
 sharded, as above) and the prompt kernel in blocks of `block_rows` rows, written into slices of preallocated outputs, and the
-layer returns (what the last-row path returned, (logprobs, ranks, top ids, top logprobs) of the rows)."""
+layer returns (what the last-row path returned, (logprobs, ranks, top ids, top logprobs) of the rows).
+
+Addition (constrained decoding, csrc/constraints.cu): when some row carries an allowed-token mask or a logit bias
+(infer_state.constraints), the logits the token is chosen from are masked and biased first, ahead of the penalties (a copy when
+log-probabilities are asked for: they stay those of the raw logits).  With a sharded lm_head the pair-merge path constrains each
+rank's shard (vocab_offset) before its local choice - a shard with no allowed id yields a -inf pair, which the merge never picks
+because the host checked that every mask allows some id; the gather path constrains the gathered full rows on every rank."""
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
+from swiftllm_b200.worker.kernels.constraints import constrain_logits
 from swiftllm_b200.worker.kernels.linear import linear
 from swiftllm_b200.worker.kernels.logprobs import prompt_logprobs, token_logprobs
 from swiftllm_b200.worker.kernels.penalties import apply_penalties
@@ -105,7 +112,7 @@ class LlamaPostLayer:
         if not already_normed:
             rmsnorm_inplace(last_input, self.weights.final_norm, self.model_config.rms_norm_eps)
         logits = linear(last_input, self.weights.lm_head)      # [batch_size, vocab_size] (or this rank's V / tp_size columns)
-        sp, n = infer_state.sampling, infer_state.logprobs
+        sp, n, con = infer_state.sampling, infer_state.logprobs, infer_state.constraints
         pen = sp is not None and sp.penalized
         sampled = sp is not None and sp.sampled
         B, Vs = logits.shape
@@ -114,14 +121,18 @@ class LlamaPostLayer:
             # them and every rank chooses the token
             full = self._gather_logits(logits) if self.sharded else logits
             if self.keep_logits:
-                self.last_logits = full.clone() if pen else full
-            chosen = self._penalised(full, infer_state, idx, copy=n is not None) if pen else full
+                self.last_logits = full.clone() if pen or con is not None else full
+            chosen = full if con is None else self._constrained(full, con, copy=n is not None)
+            if pen:
+                chosen = self._penalised(chosen, infer_state, idx, copy=n is not None and con is None)
             if sampled:
                 tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
             else:
                 tokens = torch.argmax(chosen, dim=1)
             return tokens if n is None else (tokens,) + token_logprobs(full, tokens, n)
-        raw_full = self._gather_logits(logits) if self.keep_logits and pen else None
+        raw_full = self._gather_logits(logits) if self.keep_logits and (pen or con is not None) else None
+        if con is not None:
+            self._constrained(logits, con, copy=False, vocab_offset=self.tp_rank * Vs)
         if pen:
             self._penalised(logits, infer_state, idx, copy=False, vocab_offset=self.tp_rank * Vs)
         if sampled:
@@ -138,6 +149,14 @@ class LlamaPostLayer:
         if self.keep_logits:                                   # parity tests only: reassemble the full logits
             self.last_logits = raw_full if raw_full is not None else self._gather_logits(logits)
         return merge_sharded_argmax(pairs.view(self.tp_size, B, 2))
+
+    @staticmethod
+    def _constrained(logits: torch.Tensor, con, copy: bool, vocab_offset: int = 0) -> torch.Tensor:
+        """The masked and biased logits (in place, or a copy)."""
+        out = logits.clone() if copy else logits
+        constrain_logits(out, con.mask_index, con.masks, con.bias_index, con.bias_starts, con.bias_ids, con.bias_values,
+                         vocab_offset=vocab_offset)
+        return out
 
     @staticmethod
     def _penalised(logits: torch.Tensor, infer_state: LlamaInferState, last_idx: torch.Tensor, copy: bool,

@@ -3,6 +3,7 @@
 
     LlamaModel(engine_config) -> load_weights() -> profile_num_blocks() -> init_kvcache_and_swap(num_blocks)
     forward(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False) -> list[int]
+                                                           (addition: sampling parameters, allowed-token masks)
     forward_with_logprobs(...) -> list[TokenLogprobs]      (addition: forward's arguments, tokens with log-probabilities,
                                                             and of prompt tokens with SamplingParams.prompt_logprobs)
     forward_speculative(input_ids_list, seq_ids_list, prefix_lens_list, sampling_params_list=None) -> list[list[int]]
@@ -32,14 +33,14 @@ import torch.distributed as dist
 from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
-from swiftllm_b200.sampling_params import (PromptLogprobs, SamplingParams, TokenLogprobs, has_penalties, logprobs_top_n, prompt_logprobs_top_n,
-                                           sampling_words)
+from swiftllm_b200.sampling_params import (ConstraintWords, PromptLogprobs, SamplingParams, TokenLogprobs, constraint_words,
+                                           has_penalties, logprobs_top_n, prompt_logprobs_top_n, sampling_words)
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.kernels.block_mgmt import copy_block_tails
 from swiftllm_b200.worker.weight import load_weights
 
-from .infer_state import LlamaInferState, PromptLogprobsState, SamplingState
+from .infer_state import ConstraintState, LlamaInferState, PromptLogprobsState, SamplingState
 from .layers.post_layer import LlamaPostLayer
 from .layers.pre_layer import LlamaPreLayer
 from .layers.transformer_layer import LlamaTransformerLayer
@@ -320,14 +321,15 @@ class LlamaModel:
                      decoding_lens: Optional[list], prefix=None, max_prefill_kv_len: int = 0, speculative: bool = False,
                      ignore_kvcache: bool = False, words=None, filtered: bool = False, sampled: bool = True, sampling_pos=None,
                      top_n: Optional[int] = None, prompt_state: Optional[PromptLogprobsState] = None, block_table=None,
-                     token_cache=None) -> LlamaInferState:
+                     token_cache=None, constraints=None) -> LlamaInferState:
         """The LlamaInferState of a step from its int32 device views (input ids, block-table rows, sequence lengths with the
         prefill entries first, prompt lengths and first rows, positions, rows to sample) and the sizes the host knows; the batch
         counts are the views' shapes.  decoding_lens: host decode lengths for the reference's split heuristic, None in a graph
         captured for a length bucket (the largest split).  prefix: first position of each chunk (chunked prefill, speculative
         verification), with max_prefill_kv_len.  words: staged sampling_params.sampling_words, noise counter `sampling_pos`
         (default: the sequence lengths); with penalties the sampling state also carries the token history: the input ids, the
-        block table and the token pages (default: the model's)."""
+        block table and the token pages (default: the model's).  constraints: (device view of the staged constraint region, its
+        sampling_params.ConstraintWords) or None."""
         mc = self.model_config
         B, T, P = seq_ids.shape[0], ids.shape[0], p_lens.shape[0]
         num_prefill_tokens = T - (B - P)
@@ -351,12 +353,13 @@ class LlamaModel:
             position_cos=self._cos_cached.index_select(0, pos), position_sin=self._sin_cached.index_select(0, pos),
             ignore_kvcache=ignore_kvcache, paged_attn_seq_block_size=0, last_token_indices=last,
             prefill_prefix_lens=prefix, max_prefill_kv_len=max_prefill_kv_len, speculative=speculative,
-            sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state)
+            sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state,
+            constraints=None if constraints is None else ConstraintState.from_staged(constraints[0], *constraints[1][1:]))
 
     @torch.inference_mode()
     def forward(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
                 ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
-                sampling_params_list: Optional[list] = None) -> list:
+                sampling_params_list: Optional[list] = None, token_masks_list: Optional[list] = None) -> list:
         """model.py:252-359.  Batch layout contract: prefill sequences first (full prompt each), then decoding
         sequences (exactly one token each); decoding_seq_lens_list[i] includes the new token.
 
@@ -372,26 +375,35 @@ class LlamaModel:
         None (or every temperature 0) is greedy decoding, the reference's behaviour.  Entries with repetition / frequency /
         presence penalties have their logits penalised first (csrc/penalties.cu), over the history recorded in the token pages:
         such a request must carry the same parameters from its first prefill chunk on.  Invalid parameters (and penalties with
-        ignore_kvcache, which has no block table to record into) raise ValueError before anything is enqueued."""
+        ignore_kvcache, which has no block table to record into) raise ValueError before anything is enqueued.
+
+        `token_masks_list` (addition, constrained decoding): None, or one entry per batch entry - None (unconstrained) or a packed
+        allowed-token mask, a numpy array or CPU tensor of int32 / uint32 with W = ceil(vocab_size / 32) words, bit v % 32 of word
+        v // 32 set = id v allowed (the layout of xgrammar and vLLM; swiftllm_b200.token_mask builds one; bits past vocab_size are
+        ignored).  Disallowed ids become -inf, then SamplingParams.logit_bias is added, both before the penalties
+        (csrc/constraints.cu).  A mask of the wrong shape or dtype, one that allows no id, a list of the wrong length, a bias id
+        outside [0, vocab_size) and masks with ignore_kvcache raise ValueError before anything is enqueued."""
         return self.forward_async(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache,
-                                  prefill_prefix_lens_list, sampling_params_list).tolist()
+                                  prefill_prefix_lens_list, sampling_params_list, token_masks_list).tolist()
 
     @torch.inference_mode()
     def forward_async(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False,
-                      prefill_prefix_lens_list=None, sampling_params_list=None) -> torch.Tensor:
+                      prefill_prefix_lens_list=None, sampling_params_list=None, token_masks_list=None) -> torch.Tensor:
         """Same as forward() but returns the token tensor on the device (no sync)."""
         return self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-                          sampling_params_list, with_logprobs=False)
+                          sampling_params_list, with_logprobs=False, token_masks_list=token_masks_list)
 
     @torch.inference_mode()
     def forward_with_logprobs(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
                               ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
-                              sampling_params_list: Optional[list] = None, prompt_next_ids_list: Optional[list] = None) -> list:
+                              sampling_params_list: Optional[list] = None, prompt_next_ids_list: Optional[list] = None,
+                              token_masks_list: Optional[list] = None) -> list:
         """forward() that also returns log-probabilities: one swiftllm_b200.TokenLogprobs(token, logprob, top, prompt) per batch
         entry.  Entry i gets them when sampling_params_list[i].logprobs is not None: the log-probability of its token and, for
         logprobs = N > 0, the N most likely tokens as (id, logprob), most likely first, ties broken by the smaller id.  They are
         log_softmax of the raw logits the token was chosen from (csrc/logprobs.cu), not of the temperature-scaled or filtered
-        distribution.  The tokens are the ones forward() returns for the same arguments.
+        distribution.  The tokens are the ones forward() returns for the same arguments (token_masks_list included: the
+        log-probabilities stay those of the unconstrained logits).
 
         A prefill entry with sampling_params_list[i].prompt_logprobs set also gets `prompt`, a swiftllm_b200.PromptLogprobs: each
         of its rows scores the prompt token after it (csrc/prompt_logprobs.cu, the same values as above).  The last row of the
@@ -402,7 +414,8 @@ class LlamaModel:
         plan = self._prompt_plan(input_ids_list, decoding_seq_lens_list, prefill_prefix_lens_list, sampling_params_list,
                                  prompt_next_ids_list)
         out = self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-                         sampling_params_list, with_logprobs=True, prompt_plan=plan if plan and plan["num_rows"] else None)
+                         sampling_params_list, with_logprobs=True, prompt_plan=plan if plan and plan["num_rows"] else None,
+                         token_masks_list=token_masks_list)
         prompt_out = None
         if plan and plan["num_rows"]:
             out, prompt_out = out
@@ -482,7 +495,8 @@ class LlamaModel:
 
     @torch.inference_mode()
     def forward_speculative(self, input_ids_list: list, seq_ids_list: list, prefix_lens_list: list,
-                            sampling_params_list: Optional[list] = None, ignore_kvcache: bool = False) -> list:
+                            sampling_params_list: Optional[list] = None, ignore_kvcache: bool = False,
+                            token_masks_list: Optional[list] = None) -> list:
         """Speculative decoding: score a plain decode input and up to 7 caller-made drafts per sequence in one step.
 
         Entry i is input_ids_list[i] = [x, d_1, ..., d_k] (1 <= k + 1 <= 8): x is the token a plain decode step would feed, d_* are
@@ -497,7 +511,12 @@ class LlamaModel:
         K/V of rejected rows inside a kept block are overwritten by later steps (attention never reads past a row's position).
         Speculative entries only (no prompts in the same call); runs eagerly and syncs once, like forward().  Raises ValueError
         before anything is enqueued for: a row count outside [1, 8], a negative prefix or one whose rows run past the position
-        table, ignore_kvcache, invalid sampling parameters, and penalties.  SamplingParams.logprobs is ignored."""
+        table, ignore_kvcache, invalid sampling parameters, and penalties.  SamplingParams.logprobs is ignored.
+
+        token_masks_list: None, or per entry None or a [k + 1, W] mask array (forward()'s layout, one row per input row): row j holds
+        the constraint state after x, d_1 .. d_j, the mask the caller would pass to the plain step at that position; the entry's
+        logit_bias applies to all its rows.  A draft its row's mask disallows can never equal y_j, so acceptance stops there.  A
+        mask with the wrong row count raises ValueError like forward()'s checks."""
         B = len(input_ids_list)
         if len(seq_ids_list) != B or len(prefix_lens_list) != B:
             raise ValueError(f"forward_speculative: {B} entries but {len(seq_ids_list)} seq ids and {len(prefix_lens_list)} prefixes")
@@ -514,6 +533,7 @@ class LlamaModel:
         samp = None if sampling_params_list is None else sampling_words(sampling_params_list, B, self._sampling_rng)
         if has_penalties(sampling_params_list):
             raise ValueError("forward_speculative does not apply penalties (their history is per position)")
+        con = constraint_words(token_masks_list, sampling_params_list, B, self.model_config.vocab_size, rows=rows)
         if B == 0:
             return []
         self._check_shared_writes(seq_ids_list, prefix)
@@ -529,8 +549,8 @@ class LlamaModel:
             w = np.asarray(samp[0], dtype=np.int64)
             row_words = np.concatenate([w[:2 * B].reshape(B, 2)[rep].reshape(-1)] +
                                        [w[(2 + s) * B:(3 + s) * B][rep] for s in range(3)]).tolist()
-        views = self._stage_metadata(*([row_words] if samp else []), flat_ids, seq_ids_list, seq_lengths, rows, starts,
-                                     positions, range(T), prefix, row_pos)
+        views = self._stage_metadata(*([row_words] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list,
+                                     seq_lengths, rows, starts, positions, range(T), prefix, row_pos)
         ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, p_prefix, r_pos = views[-9:]
         bm = self.gpu_block_manager
         bm.allocate_blocks_for_seqs(seq_ids, seq_lens, seq_ids_list=seq_ids_list, target_lens_list=seq_lengths,
@@ -538,7 +558,8 @@ class LlamaModel:
         infer_state = self._infer_state(ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, max_prefill_len=max(rows),
                                         max_decoding_len=0, decoding_lens=[], prefix=p_prefix,
                                         max_prefill_kv_len=max(seq_lengths), speculative=True,
-                                        words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampling_pos=r_pos)
+                                        words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampling_pos=r_pos,
+                                        constraints=None if con is None else (views[1 if samp else 0], con))
         tokens = self._forward(ids, infer_state).tolist()
         out, keep = [], []
         for ids_i, s, n_rows, p in zip(input_ids_list, starts, rows, prefix):
@@ -556,18 +577,22 @@ class LlamaModel:
         return out
 
     def _step(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-              sampling_params_list, with_logprobs: bool, prompt_plan: Optional[dict] = None):
+              sampling_params_list, with_logprobs: bool, prompt_plan: Optional[dict] = None, token_masks_list=None):
         """One step: the token tensor, or with log-probabilities asked for by some entry (with_logprobs and a
         SamplingParams.logprobs set) the tuple (tokens, token logprobs, top ids, top logprobs) on the device.  With a
         `prompt_plan` (forward_with_logprobs._prompt_plan, some rows to score): (that, (prompt logprobs, ranks, top ids, top
         logprobs)).  The step stages exactly what it stages without one: the post layer builds the rows and targets on the device
-        after the layers, so nothing of the prompt part is allocated while the forward's activations are."""
+        after the layers, so nothing of the prompt part is allocated while the forward's activations are.  token_masks_list and
+        logit_bias add the constraint region (sampling_params.constraint_words) after the sampling words; without them the step
+        stages, launches and keys its graph exactly as before."""
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
         penalized = has_penalties(sampling_params_list)
         if penalized and ignore_kvcache:
             raise ValueError("penalties need the token history of the block table: not available with ignore_kvcache")
+        if token_masks_list is not None and ignore_kvcache:
+            raise ValueError("token_masks_list does not apply to the profiling forward (ignore_kvcache)")
         sampled = samp is not None and any(sp.temperature > 0 for sp in sampling_params_list)
         num_prefill_seqs = len(input_ids_list) - len(decoding_seq_lens_list)
         flat_ids = list(itertools.chain(*input_ids_list))
@@ -593,17 +618,19 @@ class LlamaModel:
             [l - 1 for l in decoding_seq_lens_list]
         last_idx = [s + n - 1 for s, n in zip(prefill_starts, prefill_lens)] + list(range(num_prefill_tokens, num_tokens))
 
-        if (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
-                and batch_size > 0):
+        graph = (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
+                 and batch_size > 0)
+        con = constraint_words(token_masks_list, sampling_params_list, batch_size, self.model_config.vocab_size, graph=graph)
+        if graph:
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
-                                              top_n, penalized, sampled)
+                                              top_n, penalized, sampled, con)
 
         if not ignore_kvcache:
             self._check_shared_writes(seq_ids_list, prefix_lens + [l - 1 for l in decoding_seq_lens_list])
         # the sampling words go first: the int64 seeds need an 8-byte aligned offset
         views = self._stage_metadata(
-            *([samp[0]] if samp else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens, prefill_starts, positions,
-            last_idx, prefix_lens if chunked else [])
+            *([samp[0]] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens,
+            prefill_starts, positions, last_idx, prefix_lens if chunked else [])
         ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = views[-8:]
         pp = prompt_plan
         prompt_state = None if pp is None else PromptLogprobsState(
@@ -619,19 +646,21 @@ class LlamaModel:
             max_decoding_len=max_decoding_len, decoding_lens=list(decoding_seq_lens_list), prefix=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0, ignore_kvcache=ignore_kvcache,
             words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampled=sampled, top_n=top_n,
-            prompt_state=prompt_state)
+            prompt_state=prompt_state, constraints=None if con is None else (views[1 if samp else 0], con))
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
     def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
-                              sampled=True):
+                              sampled=True, con: Optional[ConstraintWords] = None):
         """Pure-decode step replayed from a CUDA graph.  The step's metadata is staged through the same pinned ring as an eager
         step's, into the graph's static device buffer, and its blocks are reserved on the manager's host mirror like an eager
         step's; the graph (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
         allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
         filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy.  A step
         with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
-        penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples)."""
+        penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples).  A
+        constrained step (`con`: the graph-sized constraint region) has its own graph per bias capacity (the step's bias entries
+        rounded up to a power of two), which also runs the constraint kernel."""
         from swiftllm_b200 import _lib
         self._check_shared_writes(seq_ids_list, [l - 1 for l in lens_list])
         B = len(flat_ids)
@@ -649,6 +678,8 @@ class LlamaModel:
             key += ("logprobs", top_n)
         if penalized:
             key += ("penalties", sampled)
+        if con is not None:
+            key += ("constrained", con.num_bias)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -656,12 +687,14 @@ class LlamaModel:
             cap = max(1, int(getattr(self.engine_config, "max_cuda_graphs", 16)))
             while len(self._graphs) >= cap:
                 self._graphs.pop(next(iter(self._graphs)))
-            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled)
+            g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled,
+                                           None if con is None else con._replace(words=None))
         self._graphs[key] = g                    # (re)insert as most recently used
         # the blocks are counted on the host, and the eager step's errors raised, before anything is enqueued; the graph's
         # allocation kernel hands them out
         self.gpu_block_manager.reserve_blocks_for_seqs(seq_ids_list, lens_list)
-        self._stage_metadata(*([samp[0]] if samp else []), flat_ids, seq_ids_list, lens_list, out=g["meta"])
+        self._stage_metadata(*([samp[0]] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list, lens_list,
+                             out=g["meta"])
         self._wait_for_swaps()
         self._penalties_used |= penalized
         g["graph"].replay()
@@ -671,15 +704,18 @@ class LlamaModel:
         return g["tokens"].clone()
 
     def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None,
-                              penalized: bool = False, sampled: bool = True):
+                              penalized: bool = False, sampled: bool = True, con: Optional[ConstraintWords] = None):
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
         also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
-        the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax."""
+        the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax.  con:
+        the sizes of the graph's constraint region (words None), which follows the sampling words; the graph constrains the
+        logits first."""
         ec = self.engine_config
         dev = self.device
         nw = 0 if filtered is None else (8 if penalized else 5) * B
-        meta = torch.zeros((nw + 3 * B,), dtype=torch.int32, device=dev)
-        ids, seq_ids, lens = meta[nw:nw + B], meta[nw + B:nw + 2 * B], meta[nw + 2 * B:]
+        nc = 0 if con is None else ConstraintWords.size(*con[1:])
+        meta = torch.zeros((nw + nc + 3 * B,), dtype=torch.int32, device=dev)
+        ids, seq_ids, lens = meta[nw + nc:nw + nc + B], meta[nw + nc + B:nw + nc + 2 * B], meta[nw + nc + 2 * B:]
         last = torch.arange(B, dtype=torch.int32, device=dev)
         empty = torch.empty((0,), dtype=torch.int32, device=dev)
 
@@ -692,7 +728,8 @@ class LlamaModel:
             st = self._infer_state(ids, seq_ids, lens, empty, empty, pos, last, max_prefill_len=0,
                                    max_decoding_len=bucket_len, decoding_lens=None,
                                    words=None if filtered is None else meta[:nw], filtered=filtered, sampled=sampled,
-                                   top_n=top_n, block_table=bm.block_table, token_cache=token_cache)
+                                   top_n=top_n, block_table=bm.block_table, token_cache=token_cache,
+                                   constraints=None if con is None else (meta[nw:nw + nc], con))
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
@@ -703,6 +740,9 @@ class LlamaModel:
         v_s = torch.zeros(sshape, dtype=self.dtype, device=dev)
         t_s = torch.zeros((B, ec.block_size), dtype=torch.int32, device=dev) if penalized else None
         meta.zero_()
+        if con is not None:
+            # warm-up region: every row on mask row 0, no bias entries, every id allowed
+            meta[nw + nc - con.num_masks * con.mask_words:nw + nc].fill_(-1)
         seq_ids.copy_(torch.arange(B, dtype=torch.int32, device=dev))
         lens.fill_(1)
         s = torch.cuda.Stream()
