@@ -13,9 +13,11 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
     ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
+    ... --lora /data/my-adapter    run every prompt under a PEFT LoRA adapter (load_lora, lora_ids_list)
 """
 import argparse
 import dataclasses
+import json
 import os
 import sys
 import time
@@ -37,6 +39,17 @@ def prompt_lookup(tokens: list, k: int, max_ngram: int = 3) -> list:
             if tokens[s:s + n] == tail:
                 return tokens[s + n:s + n + k]
     return []
+
+
+def with_adapter(model, slot: int):
+    """Every forward call of `model` runs its whole batch under LoRA adapter `slot`, except the memory-profiling forward
+    (ignore_kvcache=True, which takes no adapter): it runs the base model, whose activations are the same size."""
+    for name in ("forward", "forward_with_logprobs", "forward_speculative"):
+        def call(ids, *a, _f=getattr(model, name), **kw):
+            if kw.get("ignore_kvcache"):
+                return _f(ids, *a, **kw)
+            return _f(ids, *a, lora_ids_list=[slot] * len(ids), **kw)
+        setattr(model, name, call)
 
 
 def generate(model, input_ids, new_tokens: int, chunk: int = 0, params=None, logs=None, speculate: int = 0, n: int = 1,
@@ -148,6 +161,7 @@ def main():
     ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
     ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
     ap.add_argument("--n", type=int, default=1, help="samples per prompt: prefill once, fork n - 1 times, distinct seeds (1 = off)")
+    ap.add_argument("--lora", type=str, default=None, help="PEFT LoRA adapter directory: every prompt runs under this adapter")
     args = ap.parse_args()
     if args.n < 1:
         ap.error("--n takes a positive number of samples")
@@ -160,6 +174,10 @@ def main():
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
                                     num_cpu_blocks=0, max_seqs_in_block_table=128, max_blocks_per_seq=2048, max_batch_size=16,
                                     max_tokens_in_batch=2048 * 16, dtype=args.dtype, use_cuda_graph=args.cuda_graph)
+    if args.lora:
+        with open(os.path.join(args.lora, "adapter_config.json"), encoding="utf-8") as f:
+            r = int(json.load(f).get("r", 8))
+        ec.max_loras, ec.max_lora_rank = 1, next((k for k in (8, 16, 32, 64) if k >= r), r)
     t0 = time.perf_counter()
     if args.synthetic:
         from swiftllm_b200.model_config import LLAMA3_8B, LLAMA3_70B
@@ -179,8 +197,12 @@ def main():
                    "A B C D E F G H I J K L M N O P Q R S T U V", "To be or not to be,"]
         input_ids = tok(prompts)["input_ids"]
         show = lambda ids: tok.decode(ids, skip_special_tokens=True)
+    if args.lora:
+        model.load_lora(0, args.lora)
     num_blocks = model.profile_num_blocks()
     model.init_kvcache_and_swap(num_blocks)
+    if args.lora:
+        with_adapter(model, 0)
     print(f"{num_blocks} KV blocks; model ready in {time.perf_counter() - t0:.1f} s")
 
     params = swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs,

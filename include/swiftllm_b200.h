@@ -347,6 +347,25 @@ int sllm_constrain_logits(void* logits, int64_t num_rows, int vocab_size, int64_
                           const int32_t* bias_index, const int32_t* bias_starts, int64_t num_entries, const int32_t* bias_ids,
                           const float* bias_values, int64_t num_bias, sllm_dtype_t dtype, sllm_stream_t stream);
 
+/* ---- Multi-LoRA (new): per-request low-rank adapters added to a projection's 16-bit output y [num_rows, out_features].
+ * tiles: DEVICE int32 triples (first row, rows, slot), num_tiles of them; a tile with rows outside [1, 64], a slot outside
+ * [0, max_loras), rows past num_rows, or slice_mask[slot] == 0 is skipped (rows 0 pads a CUDA graph's fixed tile count).
+ * sllm_lora_shrink: u[t, j] = round(sum_k x[t, k] * A[j, k]) for j < u_cols, A = lora_a + slot * a_slot_stride ([u_cols,
+ * in_features] row-major, the adapter's S stacked slices of R rows), fp32 accumulation in an order fixed by in_features alone.
+ * sllm_lora_expand: y[t, n] = round(float(y[t, n]) + scales[slot] * sum_j u[t, sl * rank + j] * B[n, j]), B = lora_b + slot *
+ * b_slot_stride ([out_features, rank] row-major), sl the slice of column n ([0, slice1), [slice1, slice2), [slice2,
+ * out_features)); one fp32 multiply, one fp32 add, one rounding.  Columns of a slice whose bit (1 << sl) is clear in
+ * slice_mask[slot] are not written.  Every element of y is written by at most one thread.  Rejected before launch: unknown dtype,
+ * counts out of range, in_features not a positive multiple of 32, rank not 16 / 32 / 48 / 64, out_features or slice ends not
+ * multiples of 8, strides that do not cover a row or are misaligned, null or misaligned pointers.  num_tiles == 0 is a no-op. */
+int sllm_lora_shrink(const void* x, int64_t x_row_stride, int64_t num_rows, int in_features, void* u, int64_t u_row_stride,
+                     const void* lora_a, int64_t a_slot_stride, int u_cols, const int32_t* tiles, int64_t num_tiles,
+                     const int32_t* slice_mask, int max_loras, sllm_dtype_t dtype, sllm_stream_t stream);
+int sllm_lora_expand(void* y, int64_t y_row_stride, int64_t num_rows, int out_features, const void* u, int64_t u_row_stride,
+                     const void* lora_b, int64_t b_slot_stride, int rank, int slice1, int slice2, const int32_t* tiles,
+                     int64_t num_tiles, const int32_t* slice_mask, const float* scales, int max_loras, sllm_dtype_t dtype,
+                     sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,7 +10,8 @@ drive this LlamaModel (INTEGRATION.md).
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
 from swiftllm_b200.sampling_params import MAX_LOGIT_BIAS, PromptLogprobs, SamplingParams, TokenLogprobs, token_mask
+from swiftllm_b200.worker.lora import RANKS as LORA_RANKS, read_adapter
 from swiftllm_b200.worker.model import LlamaModel
 
 __all__ = ["EngineConfig", "LlamaModelConfig", "LlamaModel", "PromptLogprobs", "SamplingParams", "TokenLogprobs", "token_mask",
-           "MAX_LOGIT_BIAS"]
+           "MAX_LOGIT_BIAS", "LORA_RANKS", "read_adapter"]

@@ -56,6 +56,8 @@ SIGNATURES = {
     "sllm_prompt_logprobs": (_I, [_P, _L, _I, _L, _P, _I, _P, _P, _P, _P, _I, _P]),
     "sllm_apply_penalties": (_I, [_P, _L, _I, _L, _L, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _L, _I, _P]),
     "sllm_constrain_logits": (_I, [_P, _L, _I, _L, _L, _P, _P, _L, _I, _P, _P, _L, _P, _P, _L, _I, _P]),
+    "sllm_lora_shrink": (_I, [_P, _L, _L, _I, _P, _L, _P, _L, _I, _P, _L, _P, _I, _I, _P]),
+    "sllm_lora_expand": (_I, [_P, _L, _L, _I, _P, _L, _P, _L, _I, _I, _I, _P, _L, _P, _P, _I, _I, _P]),
 }
 
 _lib = None

@@ -55,6 +55,10 @@ class EngineConfig:
     # seeds the generator that gives SamplingParams(seed=None) rows a fresh seed each step: runs are reproducible, repeated
     # prompts still vary
     sampling_seed: int = 0
+    # multi-LoRA (worker/lora.py): adapter slots loaded with LlamaModel.load_lora and chosen per batch entry (lora_ids_list), and
+    # their largest rank, one of 8, 16, 32, 64 (storage padded to a multiple of 16).  max_loras 0: nothing is allocated
+    max_loras: int = 0
+    max_lora_rank: int = 0
 
     @staticmethod
     def add_cli_args(parser: argparse.ArgumentParser):

@@ -63,6 +63,14 @@ class LlamaInferState:
     # Allowed-token masks and logit bias of the step's last rows (csrc/constraints.cu); None = no row is constrained.  Kept apart
     # from `sampling`: a constrained step may be greedy with no sampling parameters at all
     constraints: Optional["ConstraintState"] = None
+    # Per-request LoRA adapters (worker/lora.py, csrc/lora.cu): the slot pool and the step's tile list; None = no row is adapted
+    lora: Optional["LoraState"] = None
+
+
+@dataclasses.dataclass
+class LoraState:
+    pool: object                    # worker.lora.LoraPool
+    tiles: torch.Tensor             # [num_tiles, 3] int32 (first row, rows, slot); rows 0 pads a graph's fixed tile count
 
 
 @dataclasses.dataclass

@@ -7,6 +7,10 @@ Differences by design: the prefill attention is this library's own kernel (the r
 vllm_flash_attn, :86-96); with tensor parallelism each rank runs its head / FFN-column shard and the partial
 o_proj / down_proj outputs are summed with ONE NCCL all-reduce each (the only collectives of the model); the
 side stream for decode attention (:103-114) is only used when the batch really mixes prefill and decode work.
+
+Per-request LoRA adapters (infer_state.lora, worker/lora.py): right after each of the four GEMMs (qkv, o, up_gate, down) a
+shrink and an expand launch add the adapters' deltas into the GEMM output in place - under TP into the rank's partial output
+(the NCCL buffer or comm.partial_out) before the exchange sums the ranks.
 """
 import torch
 import torch.distributed as dist
@@ -14,6 +18,7 @@ import torch.distributed as dist
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.kvcache_mgmt import rotary_store_kvcache_decode, store_kvcache
 from swiftllm_b200.worker.kernels.linear import linear
+from swiftllm_b200.worker.kernels.lora import lora_expand, lora_shrink
 from swiftllm_b200.worker.kernels.paged_attn import paged_attention
 from swiftllm_b200.worker.kernels.prefill_attn import paged_attention_verify, prefill_attention, prefill_attention_paged
 from swiftllm_b200.worker.kernels.rmsnorm import fused_add_rmsnorm_inplace
@@ -41,6 +46,15 @@ class LlamaTransformerLayer:
         if self.tp_size > 1:
             dist.all_reduce(x, group=self.tp_group)
 
+    def _lora(self, lora, site: int, x: torch.Tensor, y: torch.Tensor):
+        """y += the step's adapter deltas at `site` (worker.lora.SITES index); nothing when the step has no adapter."""
+        if lora is None:
+            return
+        p = lora.pool
+        mask = p.slice_mask[self.layer_id, site]
+        lora_shrink(x, p.u, p.a[self.layer_id][site], lora.tiles, mask)
+        lora_expand(y, p.u, p.b[self.layer_id][site], p.dims_ends[site], lora.tiles, mask, p.scales)
+
     def forward(
         self,
         input_embds: torch.Tensor,  # [num_tokens, hidden_size]
@@ -62,6 +76,8 @@ class LlamaTransformerLayer:
         # one GEMM for q, k and v (three latency-bound GEMMs in the reference, transformer_layer.py:54-56); the
         # kernels below take the row-strided column slices directly
         qkv = linear(input_embds, w.qkv_proj)
+        lora = infer_state.lora
+        self._lora(lora, 0, input_embds, qkv)
         T, nqd, nkvd = qkv.shape[0], self.num_q_heads * mc.head_dim, self.num_kv_heads * mc.head_dim
         q = qkv[:, :nqd].unflatten(1, (self.num_q_heads, mc.head_dim))
         k = qkv[:, nqd:nqd + nkvd].unflatten(1, (self.num_kv_heads, mc.head_dim))
@@ -108,19 +124,26 @@ class LlamaTransformerLayer:
         if comm is not None:
             T = o.shape[0]
             torch.mm(o, w.o_proj.t(), out=comm.partial_out(0, T))              # partial sums -> symmetric buffer 0
+            self._lora(lora, 1, o, comm.partial_out(0, T))
             o = comm.reduce_add_norm(0, T, residual_buf, w.ffn_norm, mc.rms_norm_eps)
             up_gate_proj = linear(o, w.up_gate_proj)
+            self._lora(lora, 2, o, up_gate_proj)
             silu_and_mul_inplace(up_gate_proj)
             ffn_out = comm.partial_out(1, T)                                   # consumed by the next layer / the model tail
             torch.mm(up_gate_proj[:, :self.ffn_inter_dim], w.down_proj.t(), out=ffn_out)
+            self._lora(lora, 3, up_gate_proj[:, :self.ffn_inter_dim], ffn_out)
             return ffn_out
 
+        attn = o
         o = linear(o, w.o_proj)                # row-parallel under TP: partial sums
+        self._lora(lora, 1, attn, o)
         self._all_reduce(o)
         fused_add_rmsnorm_inplace(o, residual_buf, w.ffn_norm, mc.rms_norm_eps)
 
         up_gate_proj = linear(o, w.up_gate_proj)
+        self._lora(lora, 2, o, up_gate_proj)
         silu_and_mul_inplace(up_gate_proj)
         ffn_out = linear(up_gate_proj[:, :self.ffn_inter_dim], w.down_proj)
+        self._lora(lora, 3, up_gate_proj[:, :self.ffn_inter_dim], ffn_out)
         self._all_reduce(ffn_out)
         return ffn_out

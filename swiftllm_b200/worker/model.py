@@ -9,6 +9,7 @@
     forward_speculative(input_ids_list, seq_ids_list, prefix_lens_list, sampling_params_list=None) -> list[list[int]]
                                                             (addition: verify up to 7 drafts per sequence in one step)
     fork_seqs(src_seq_ids_list, dst_seq_ids_list, lens_list)  (addition: share a cached prefix with another sequence)
+    load_lora(slot, adapter) / unload_lora(slot)               (addition: per-request LoRA adapters, lora_ids_list)
     swap_in_seqs / swap_out_seqs / free_seqs_resources
 
 and the same observable state (k_cache, v_cache, k_swap, v_swap, gpu_block_manager, cpu_block_manager).  Addition: the token
@@ -38,9 +39,10 @@ from swiftllm_b200.sampling_params import (ConstraintWords, PromptLogprobs, Samp
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.kernels.block_mgmt import copy_block_tails
+from swiftllm_b200.worker.lora import LoraPool, lora_tiles
 from swiftllm_b200.worker.weight import load_weights
 
-from .infer_state import ConstraintState, LlamaInferState, PromptLogprobsState, SamplingState
+from .infer_state import ConstraintState, LlamaInferState, LoraState, PromptLogprobsState, SamplingState
 from .layers.post_layer import LlamaPostLayer
 from .layers.pre_layer import LlamaPreLayer
 from .layers.transformer_layer import LlamaTransformerLayer
@@ -113,6 +115,7 @@ class LlamaModel:
         self._penalties_used = False
         self.cpu_block_manager = self.gpu_block_manager = None
         self.tp_group = None
+        self.lora = None                # LoraPool (EngineConfig.max_loras > 0)
         self._graphs = {}
         # pinned staging ring for per-step metadata (every step path): a slot is rewritten only after the H2D copy that last read it
         # has completed (event per slot), so back-to-back forward_async calls never race the copy engine
@@ -176,6 +179,55 @@ class LlamaModel:
         ]
         self.post_layer = LlamaPostLayer(self.model_config, self.weight, tp_group=self.tp_group, tp_rank=self.tp_rank,
                                          tp_size=self.tp_size)
+        ec = self.engine_config
+        if getattr(ec, "max_loras", 0):
+            # allocated before profile_num_blocks, so the KV-cache sizing leaves room for it
+            self.lora = LoraPool(self.model_config, ec.max_loras, getattr(ec, "max_lora_rank", 0), self.dtype, self.device,
+                                 ec.max_tokens_in_batch, tp_rank=self.tp_rank, tp_size=self.tp_size)
+            print(f"[Model.lora] {ec.max_loras} adapter slots of rank {self.lora.rank}: {self.lora.nbytes() / GB:.3f} GB "
+                  f"({self.lora.nbytes() / ec.max_loras / 2 ** 20:.1f} MiB per slot)")
+
+    # ------------------------------------------------------------------ LoRA adapters
+    @torch.inference_mode()
+    def load_lora(self, slot: int, adapter):
+        """Copy a PEFT LoRA adapter into slot `slot` (replacing what it held); requests choose it with lora_ids_list.  `adapter`
+        is a PEFT adapter directory (adapter_config.json + adapter_model.safetensors or adapter_model.bin) or a (config dict,
+        {PEFT key: tensor}) pair.  Read keys: base_model.model.model.layers.{i}.{self_attn,mlp}.{q,k,v,o,gate,up,down}_proj
+        .lora_{A,B}.weight, A [r, in], B [out, r]; scale lora_alpha / r (lora_alpha / sqrt(r) with use_rslora); tensors are
+        rounded once to the model dtype.  Modules the adapter leaves out keep the base model's outputs bit for bit.  Raises
+        ValueError before anything is copied for: max_loras 0, a slot outside [0, max_loras), r > max_lora_rank, a shape that
+        does not match the model, fan_in_fan_out, bias other than "none", DoRA, a non-empty rank_pattern / alpha_pattern /
+        modules_to_save / layers_to_transform, adapters on embed_tokens or lm_head, and tensors under any other key.  Each
+        tensor-parallel rank loads the same adapter and keeps its slices."""
+        if self.lora is None:
+            raise ValueError("load_lora: the engine has no adapter slots (EngineConfig.max_loras is 0)")
+        self.lora.load(slot, adapter)
+
+    @torch.inference_mode()
+    def unload_lora(self, slot: int):
+        """Empty slot `slot`: requests may no longer name it."""
+        if self.lora is None:
+            raise ValueError("unload_lora: the engine has no adapter slots (EngineConfig.max_loras is 0)")
+        self.lora.unload(slot)
+
+    def _lora_slots(self, lora_ids_list, batch_size: int, ignore_kvcache: bool) -> Optional[list]:
+        """The validated per-entry slots, or None when no entry is adapted (the step is then exactly the unadapted one)."""
+        if lora_ids_list is None:
+            return None
+        if ignore_kvcache:
+            raise ValueError("lora_ids_list does not apply to the profiling forward (ignore_kvcache)")
+        if len(lora_ids_list) != batch_size:
+            raise ValueError(f"lora_ids_list has {len(lora_ids_list)} entries for {batch_size} batch entries")
+        slots = []
+        for i, s in enumerate(lora_ids_list):
+            if s is not None:
+                if isinstance(s, bool) or not isinstance(s, (int, np.integer)):
+                    raise ValueError(f"lora_ids_list[{i}] must be None or a slot id, got {s!r}")
+                s = int(s)
+                if self.lora is None or not 0 <= s < self.lora.max_loras or not self.lora.loaded[s]:
+                    raise ValueError(f"lora_ids_list[{i}]: adapter slot {s} is not loaded")
+            slots.append(s)
+        return slots if any(s is not None for s in slots) else None
 
     def _shard_lm_head(self) -> bool:
         want = getattr(self.engine_config, "shard_lm_head", None)
@@ -321,7 +373,7 @@ class LlamaModel:
                      decoding_lens: Optional[list], prefix=None, max_prefill_kv_len: int = 0, speculative: bool = False,
                      ignore_kvcache: bool = False, words=None, filtered: bool = False, sampled: bool = True, sampling_pos=None,
                      top_n: Optional[int] = None, prompt_state: Optional[PromptLogprobsState] = None, block_table=None,
-                     token_cache=None, constraints=None) -> LlamaInferState:
+                     token_cache=None, constraints=None, lora_tiles_view=None) -> LlamaInferState:
         """The LlamaInferState of a step from its int32 device views (input ids, block-table rows, sequence lengths with the
         prefill entries first, prompt lengths and first rows, positions, rows to sample) and the sizes the host knows; the batch
         counts are the views' shapes.  decoding_lens: host decode lengths for the reference's split heuristic, None in a graph
@@ -329,7 +381,7 @@ class LlamaModel:
         verification), with max_prefill_kv_len.  words: staged sampling_params.sampling_words, noise counter `sampling_pos`
         (default: the sequence lengths); with penalties the sampling state also carries the token history: the input ids, the
         block table and the token pages (default: the model's).  constraints: (device view of the staged constraint region, its
-        sampling_params.ConstraintWords) or None."""
+        sampling_params.ConstraintWords) or None.  lora_tiles_view: the staged LoRA tile words or None."""
         mc = self.model_config
         B, T, P = seq_ids.shape[0], ids.shape[0], p_lens.shape[0]
         num_prefill_tokens = T - (B - P)
@@ -354,12 +406,14 @@ class LlamaModel:
             ignore_kvcache=ignore_kvcache, paged_attn_seq_block_size=0, last_token_indices=last,
             prefill_prefix_lens=prefix, max_prefill_kv_len=max_prefill_kv_len, speculative=speculative,
             sampling=sampling, logprobs=top_n, prompt_logprobs=prompt_state,
-            constraints=None if constraints is None else ConstraintState.from_staged(constraints[0], *constraints[1][1:]))
+            constraints=None if constraints is None else ConstraintState.from_staged(constraints[0], *constraints[1][1:]),
+            lora=None if lora_tiles_view is None else LoraState(self.lora, lora_tiles_view.view(-1, 3)))
 
     @torch.inference_mode()
     def forward(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
                 ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
-                sampling_params_list: Optional[list] = None, token_masks_list: Optional[list] = None) -> list:
+                sampling_params_list: Optional[list] = None, token_masks_list: Optional[list] = None,
+                lora_ids_list: Optional[list] = None) -> list:
         """model.py:252-359.  Batch layout contract: prefill sequences first (full prompt each), then decoding
         sequences (exactly one token each); decoding_seq_lens_list[i] includes the new token.
 
@@ -382,22 +436,30 @@ class LlamaModel:
         v // 32 set = id v allowed (the layout of xgrammar and vLLM; swiftllm_b200.token_mask builds one; bits past vocab_size are
         ignored).  Disallowed ids become -inf, then SamplingParams.logit_bias is added, both before the penalties
         (csrc/constraints.cu).  A mask of the wrong shape or dtype, one that allows no id, a list of the wrong length, a bias id
-        outside [0, vocab_size) and masks with ignore_kvcache raise ValueError before anything is enqueued."""
+        outside [0, vocab_size) and masks with ignore_kvcache raise ValueError before anything is enqueued.
+
+        `lora_ids_list` (addition, multi-LoRA): None, or one entry per batch entry - None (the base model) or a slot loaded with
+        load_lora; the entry's rows run with that adapter at every projection (csrc/lora.cu).  K/V cached by an adapted entry
+        depend on its adapter: keep a sequence on one slot (and fork it only to sequences of the same slot).  A list of the wrong
+        length, a slot that is not loaded and use with ignore_kvcache raise ValueError before anything is enqueued.  A list of
+        None entries is a step without adapters."""
         return self.forward_async(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache,
-                                  prefill_prefix_lens_list, sampling_params_list, token_masks_list).tolist()
+                                  prefill_prefix_lens_list, sampling_params_list, token_masks_list, lora_ids_list).tolist()
 
     @torch.inference_mode()
     def forward_async(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache=False,
-                      prefill_prefix_lens_list=None, sampling_params_list=None, token_masks_list=None) -> torch.Tensor:
+                      prefill_prefix_lens_list=None, sampling_params_list=None, token_masks_list=None,
+                      lora_ids_list=None) -> torch.Tensor:
         """Same as forward() but returns the token tensor on the device (no sync)."""
         return self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-                          sampling_params_list, with_logprobs=False, token_masks_list=token_masks_list)
+                          sampling_params_list, with_logprobs=False, token_masks_list=token_masks_list,
+                          lora_ids_list=lora_ids_list)
 
     @torch.inference_mode()
     def forward_with_logprobs(self, input_ids_list: list, seq_ids_list: list, decoding_seq_lens_list: list,
                               ignore_kvcache: bool = False, prefill_prefix_lens_list: Optional[list] = None,
                               sampling_params_list: Optional[list] = None, prompt_next_ids_list: Optional[list] = None,
-                              token_masks_list: Optional[list] = None) -> list:
+                              token_masks_list: Optional[list] = None, lora_ids_list: Optional[list] = None) -> list:
         """forward() that also returns log-probabilities: one swiftllm_b200.TokenLogprobs(token, logprob, top, prompt) per batch
         entry.  Entry i gets them when sampling_params_list[i].logprobs is not None: the log-probability of its token and, for
         logprobs = N > 0, the N most likely tokens as (id, logprob), most likely first, ties broken by the smaller id.  They are
@@ -410,12 +472,13 @@ class LlamaModel:
         entry scores prompt_next_ids_list[i] when that is given (one entry per prefill entry, None or the id of the prompt token
         after this chunk); so chunks of a prompt, each given the next chunk's first token, together score positions 1 .. P - 1.
         The step's tokens and KV-cache writes are those of forward().  A prompt_next_ids_list of the wrong length, or an id of an
-        asking entry outside [0, vocab_size), raises ValueError before anything is enqueued."""
+        asking entry outside [0, vocab_size), raises ValueError before anything is enqueued.  With lora_ids_list, every
+        log-probability (prompt ones included) is the adapted model's."""
         plan = self._prompt_plan(input_ids_list, decoding_seq_lens_list, prefill_prefix_lens_list, sampling_params_list,
                                  prompt_next_ids_list)
         out = self._step(input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
                          sampling_params_list, with_logprobs=True, prompt_plan=plan if plan and plan["num_rows"] else None,
-                         token_masks_list=token_masks_list)
+                         token_masks_list=token_masks_list, lora_ids_list=lora_ids_list)
         prompt_out = None
         if plan and plan["num_rows"]:
             out, prompt_out = out
@@ -496,7 +559,7 @@ class LlamaModel:
     @torch.inference_mode()
     def forward_speculative(self, input_ids_list: list, seq_ids_list: list, prefix_lens_list: list,
                             sampling_params_list: Optional[list] = None, ignore_kvcache: bool = False,
-                            token_masks_list: Optional[list] = None) -> list:
+                            token_masks_list: Optional[list] = None, lora_ids_list: Optional[list] = None) -> list:
         """Speculative decoding: score a plain decode input and up to 7 caller-made drafts per sequence in one step.
 
         Entry i is input_ids_list[i] = [x, d_1, ..., d_k] (1 <= k + 1 <= 8): x is the token a plain decode step would feed, d_* are
@@ -516,7 +579,8 @@ class LlamaModel:
         token_masks_list: None, or per entry None or a [k + 1, W] mask array (forward()'s layout, one row per input row): row j holds
         the constraint state after x, d_1 .. d_j, the mask the caller would pass to the plain step at that position; the entry's
         logit_bias applies to all its rows.  A draft its row's mask disallows can never equal y_j, so acceptance stops there.  A
-        mask with the wrong row count raises ValueError like forward()'s checks."""
+        mask with the wrong row count raises ValueError like forward()'s checks.  lora_ids_list: forward()'s, one slot per
+        entry, shared by all its rows."""
         B = len(input_ids_list)
         if len(seq_ids_list) != B or len(prefix_lens_list) != B:
             raise ValueError(f"forward_speculative: {B} entries but {len(seq_ids_list)} seq ids and {len(prefix_lens_list)} prefixes")
@@ -534,6 +598,7 @@ class LlamaModel:
         if has_penalties(sampling_params_list):
             raise ValueError("forward_speculative does not apply penalties (their history is per position)")
         con = constraint_words(token_masks_list, sampling_params_list, B, self.model_config.vocab_size, rows=rows)
+        slots = self._lora_slots(lora_ids_list, B, False)
         if B == 0:
             return []
         self._check_shared_writes(seq_ids_list, prefix)
@@ -549,8 +614,12 @@ class LlamaModel:
             w = np.asarray(samp[0], dtype=np.int64)
             row_words = np.concatenate([w[:2 * B].reshape(B, 2)[rep].reshape(-1)] +
                                        [w[(2 + s) * B:(3 + s) * B][rep] for s in range(3)]).tolist()
-        views = self._stage_metadata(*([row_words] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list,
-                                     seq_lengths, rows, starts, positions, range(T), prefix, row_pos)
+        tiles = None if slots is None else lora_tiles(slots, rows)
+        if tiles is not None:
+            self.lora.ensure_rows(T)
+        views = self._stage_metadata(*([row_words] if samp else []), *([con.words] if con else []),
+                                     *([tiles] if tiles else []), flat_ids, seq_ids_list, seq_lengths, rows, starts, positions,
+                                     range(T), prefix, row_pos)
         ids, seq_ids, seq_lens, p_lens, p_starts, pos, last, p_prefix, r_pos = views[-9:]
         bm = self.gpu_block_manager
         bm.allocate_blocks_for_seqs(seq_ids, seq_lens, seq_ids_list=seq_ids_list, target_lens_list=seq_lengths,
@@ -559,7 +628,8 @@ class LlamaModel:
                                         max_decoding_len=0, decoding_lens=[], prefix=p_prefix,
                                         max_prefill_kv_len=max(seq_lengths), speculative=True,
                                         words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampling_pos=r_pos,
-                                        constraints=None if con is None else (views[1 if samp else 0], con))
+                                        constraints=None if con is None else (views[1 if samp else 0], con),
+                                        lora_tiles_view=views[bool(samp) + bool(con)] if tiles else None)
         tokens = self._forward(ids, infer_state).tolist()
         out, keep = [], []
         for ids_i, s, n_rows, p in zip(input_ids_list, starts, rows, prefix):
@@ -577,14 +647,15 @@ class LlamaModel:
         return out
 
     def _step(self, input_ids_list, seq_ids_list, decoding_seq_lens_list, ignore_kvcache, prefill_prefix_lens_list,
-              sampling_params_list, with_logprobs: bool, prompt_plan: Optional[dict] = None, token_masks_list=None):
+              sampling_params_list, with_logprobs: bool, prompt_plan: Optional[dict] = None, token_masks_list=None,
+              lora_ids_list=None):
         """One step: the token tensor, or with log-probabilities asked for by some entry (with_logprobs and a
         SamplingParams.logprobs set) the tuple (tokens, token logprobs, top ids, top logprobs) on the device.  With a
         `prompt_plan` (forward_with_logprobs._prompt_plan, some rows to score): (that, (prompt logprobs, ranks, top ids, top
         logprobs)).  The step stages exactly what it stages without one: the post layer builds the rows and targets on the device
         after the layers, so nothing of the prompt part is allocated while the forward's activations are.  token_masks_list and
         logit_bias add the constraint region (sampling_params.constraint_words) after the sampling words; without them the step
-        stages, launches and keys its graph exactly as before."""
+        stages, launches and keys its graph exactly as before; so does lora_ids_list with the LoRA tile list (after those)."""
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
@@ -593,6 +664,7 @@ class LlamaModel:
             raise ValueError("penalties need the token history of the block table: not available with ignore_kvcache")
         if token_masks_list is not None and ignore_kvcache:
             raise ValueError("token_masks_list does not apply to the profiling forward (ignore_kvcache)")
+        slots = self._lora_slots(lora_ids_list, len(input_ids_list), ignore_kvcache)
         sampled = samp is not None and any(sp.temperature > 0 for sp in sampling_params_list)
         num_prefill_seqs = len(input_ids_list) - len(decoding_seq_lens_list)
         flat_ids = list(itertools.chain(*input_ids_list))
@@ -621,16 +693,19 @@ class LlamaModel:
         graph = (getattr(self.engine_config, "use_cuda_graph", False) and num_prefill_seqs == 0 and not ignore_kvcache
                  and batch_size > 0)
         con = constraint_words(token_masks_list, sampling_params_list, batch_size, self.model_config.vocab_size, graph=graph)
+        if slots is not None:
+            self.lora.ensure_rows(num_tokens)
         if graph:
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
-                                              top_n, penalized, sampled, con)
+                                              top_n, penalized, sampled, con, slots)
+        tiles = None if slots is None else lora_tiles(slots, prefill_lens + [1] * (batch_size - num_prefill_seqs))
 
         if not ignore_kvcache:
             self._check_shared_writes(seq_ids_list, prefix_lens + [l - 1 for l in decoding_seq_lens_list])
         # the sampling words go first: the int64 seeds need an 8-byte aligned offset
         views = self._stage_metadata(
-            *([samp[0]] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list, seq_lengths_list, prefill_lens,
-            prefill_starts, positions, last_idx, prefix_lens if chunked else [])
+            *([samp[0]] if samp else []), *([con.words] if con else []), *([tiles] if tiles else []), flat_ids, seq_ids_list,
+            seq_lengths_list, prefill_lens, prefill_starts, positions, last_idx, prefix_lens if chunked else [])
         ids, seq_ids, seq_lengths, p_lens, p_starts, pos, last, p_prefix = views[-8:]
         pp = prompt_plan
         prompt_state = None if pp is None else PromptLogprobsState(
@@ -646,12 +721,13 @@ class LlamaModel:
             max_decoding_len=max_decoding_len, decoding_lens=list(decoding_seq_lens_list), prefix=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0, ignore_kvcache=ignore_kvcache,
             words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampled=sampled, top_n=top_n,
-            prompt_state=prompt_state, constraints=None if con is None else (views[1 if samp else 0], con))
+            prompt_state=prompt_state, constraints=None if con is None else (views[1 if samp else 0], con),
+            lora_tiles_view=views[bool(samp) + bool(con)] if tiles else None)
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
     def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
-                              sampled=True, con: Optional[ConstraintWords] = None):
+                              sampled=True, con: Optional[ConstraintWords] = None, slots: Optional[list] = None):
         """Pure-decode step replayed from a CUDA graph.  The step's metadata is staged through the same pinned ring as an eager
         step's, into the graph's static device buffer, and its blocks are reserved on the manager's host mirror like an eager
         step's; the graph (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
@@ -660,7 +736,8 @@ class LlamaModel:
         with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
         penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples).  A
         constrained step (`con`: the graph-sized constraint region) has its own graph per bias capacity (the step's bias entries
-        rounded up to a power of two), which also runs the constraint kernel."""
+        rounded up to a power of two), which also runs the constraint kernel.  An adapted step (`slots`, _lora_slots) has its own
+        graph, which also runs the LoRA kernels over a tile list padded to B tiles, so any mix of slots replays it."""
         from swiftllm_b200 import _lib
         self._check_shared_writes(seq_ids_list, [l - 1 for l in lens_list])
         B = len(flat_ids)
@@ -680,6 +757,8 @@ class LlamaModel:
             key += ("penalties", sampled)
         if con is not None:
             key += ("constrained", con.num_bias)
+        if slots is not None:
+            key += ("lora",)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -688,13 +767,15 @@ class LlamaModel:
             while len(self._graphs) >= cap:
                 self._graphs.pop(next(iter(self._graphs)))
             g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled,
-                                           None if con is None else con._replace(words=None))
+                                           None if con is None else con._replace(words=None),
+                                           **({} if slots is None else dict(lora=True)))
         self._graphs[key] = g                    # (re)insert as most recently used
         # the blocks are counted on the host, and the eager step's errors raised, before anything is enqueued; the graph's
         # allocation kernel hands them out
         self.gpu_block_manager.reserve_blocks_for_seqs(seq_ids_list, lens_list)
-        self._stage_metadata(*([samp[0]] if samp else []), *([con.words] if con else []), flat_ids, seq_ids_list, lens_list,
-                             out=g["meta"])
+        tiles = [] if slots is None else lora_tiles(slots, [1] * B, pad_to=B)
+        self._stage_metadata(*([samp[0]] if samp else []), *([con.words] if con else []), *([tiles] if tiles else []), flat_ids,
+                             seq_ids_list, lens_list, out=g["meta"])
         self._wait_for_swaps()
         self._penalties_used |= penalized
         g["graph"].replay()
@@ -704,18 +785,21 @@ class LlamaModel:
         return g["tokens"].clone()
 
     def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None,
-                              penalized: bool = False, sampled: bool = True, con: Optional[ConstraintWords] = None):
+                              penalized: bool = False, sampled: bool = True, con: Optional[ConstraintWords] = None,
+                              lora: bool = False):
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
         also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
         the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax.  con:
         the sizes of the graph's constraint region (words None), which follows the sampling words; the graph constrains the
-        logits first."""
+        logits first.  lora: B LoRA tiles follow (empty during the warm-up)."""
         ec = self.engine_config
         dev = self.device
         nw = 0 if filtered is None else (8 if penalized else 5) * B
         nc = 0 if con is None else ConstraintWords.size(*con[1:])
-        meta = torch.zeros((nw + nc + 3 * B,), dtype=torch.int32, device=dev)
-        ids, seq_ids, lens = meta[nw + nc:nw + nc + B], meta[nw + nc + B:nw + nc + 2 * B], meta[nw + nc + 2 * B:]
+        nl = 3 * B if lora else 0
+        meta = torch.zeros((nw + nc + nl + 3 * B,), dtype=torch.int32, device=dev)
+        o = nw + nc + nl
+        ids, seq_ids, lens = meta[o:o + B], meta[o + B:o + 2 * B], meta[o + 2 * B:]
         last = torch.arange(B, dtype=torch.int32, device=dev)
         empty = torch.empty((0,), dtype=torch.int32, device=dev)
 
@@ -729,7 +813,8 @@ class LlamaModel:
                                    max_decoding_len=bucket_len, decoding_lens=None,
                                    words=None if filtered is None else meta[:nw], filtered=filtered, sampled=sampled,
                                    top_n=top_n, block_table=bm.block_table, token_cache=token_cache,
-                                   constraints=None if con is None else (meta[nw:nw + nc], con))
+                                   constraints=None if con is None else (meta[nw:nw + nc], con),
+                                   lora_tiles_view=meta[nw + nc:o] if lora else None)
             return self._forward(ids, st, k_cache=k_cache, v_cache=v_cache, block_table=bm.block_table)
 
         # Warm-up (library handles, lazy kernel loading, GEMM heuristics for these shapes) must not touch the real
@@ -760,8 +845,10 @@ class LlamaModel:
             out = step(self.gpu_block_manager, self.k_cache, self.v_cache, self.token_cache)
         torch.cuda.synchronize()
         tokens, logprobs = (out, None) if top_n is None else (out[0], out[1:])
-        # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph
-        return dict(graph=graph, meta=meta, tokens=tokens, logprobs=logprobs, keep=(last, empty))
+        # `last` / `empty` are read by the captured kernels on every replay: keep them alive with the graph, and
+        # the LoRA u buffer too: LoraPool.ensure_rows may replace it, and this graph reads the one it was captured with
+        return dict(graph=graph, meta=meta, tokens=tokens, logprobs=logprobs,
+                    keep=(last, empty) + ((self.lora.u,) if lora else ()))
 
     # ------------------------------------------------------------------ shared blocks
     def _check_shared_writes(self, seq_ids_list, first_positions):
@@ -794,7 +881,10 @@ class LlamaModel:
         freed when its last owner is freed or swapped out, and a swapped-out fork comes back with private blocks.  Raises
         ValueError, before anything is enqueued, when the list lengths differ, P < 1 or P > blocks held by src * block_size, src
         holds no GPU blocks (or is swapped out), dst holds blocks on either device, a dst repeats or is also a src, or an id is
-        outside [0, max_seqs_in_block_table); RuntimeError when the tail blocks do not fit.  Stream-ordered, no host sync."""
+        outside [0, max_seqs_in_block_table); RuntimeError when the tail blocks do not fit.  Stream-ordered, no host sync.
+
+        Cached K/V depend on the LoRA adapter that computed them (lora_ids_list): fork only to sequences that continue with the
+        source's slot.  The data plane cannot detect a fork across adapters."""
         B = len(src_seq_ids_list)
         if len(dst_seq_ids_list) != B or len(lens_list) != B:
             raise ValueError(f"fork_seqs: {B} sources but {len(dst_seq_ids_list)} destinations and {len(lens_list)} lengths")
