@@ -14,6 +14,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
     ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
     ... --lora /data/my-adapter    run every prompt under a PEFT LoRA adapter (load_lora, lora_ids_list)
+    ... --quantization fp8 e4m3 projection weights (16-bit checkpoints are quantized at load; FP8 checkpoints load as they are)
 """
 import argparse
 import dataclasses
@@ -162,6 +163,8 @@ def main():
     ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
     ap.add_argument("--n", type=int, default=1, help="samples per prompt: prefill once, fork n - 1 times, distinct seeds (1 = off)")
     ap.add_argument("--lora", type=str, default=None, help="PEFT LoRA adapter directory: every prompt runs under this adapter")
+    ap.add_argument("--quantization", type=str, default=None, choices=["fp8"],
+                    help="fp8: e4m3 projection weights, 16-bit checkpoints quantized at load (default: follow the checkpoint)")
     args = ap.parse_args()
     if args.n < 1:
         ap.error("--n takes a positive number of samples")
@@ -173,7 +176,8 @@ def main():
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
                                     num_cpu_blocks=0, max_seqs_in_block_table=128, max_blocks_per_seq=2048, max_batch_size=16,
-                                    max_tokens_in_batch=2048 * 16, dtype=args.dtype, use_cuda_graph=args.cuda_graph)
+                                    max_tokens_in_batch=2048 * 16, dtype=args.dtype, use_cuda_graph=args.cuda_graph,
+                                    quantization=args.quantization)
     if args.lora:
         with open(os.path.join(args.lora, "adapter_config.json"), encoding="utf-8") as f:
             r = int(json.load(f).get("r", 8))

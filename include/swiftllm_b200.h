@@ -366,6 +366,22 @@ int sllm_lora_expand(void* y, int64_t y_row_stride, int64_t num_rows, int out_fe
                      int64_t num_tiles, const int32_t* slice_mask, const float* scales, int max_loras, sllm_dtype_t dtype,
                      sllm_stream_t stream);
 
+/* ---- FP8 weights (new): per-token e4m3 quantization of GEMM inputs, one CTA per row.  For a row y of the storage dtype:
+ * s = fmaxf(amax(|y|) / 448.f, 0x1p-126f) (fp32, IEEE division), q_j = e4m3 round-to-nearest-even with saturation to +-448 of
+ * y_j / s (fp32 IEEE division), so y_j ~= q_j * s.  Outputs: q (e4m3 bytes, [rows, cols] row-major) and scales (fp32 [rows]).
+ * sllm_fused_add_rmsnorm_quant_fp8: y = the fused add+RMSNorm row of sllm_fused_add_rmsnorm_inplace (the residual is updated
+ * exactly as there); x is read, not written.  sllm_silu_and_mul_quant_fp8: y = sllm_silu_and_mul_inplace's row of [up | gate]
+ * (x read, not written; row stride >= 2F).  sllm_quant_fp8_rows: y = the given rows (row stride x_row_stride elements).
+ * Rejected before launch: unknown dtype, a row length not a positive multiple of 16 (up to 65536 for the first two), counts >=
+ * 2^31, strides that do not cover a row or are not multiples of 8, null or misaligned pointers (16-bit operands 16-byte, q
+ * 8-byte aligned).  Zero rows are a no-op. */
+int sllm_fused_add_rmsnorm_quant_fp8(const void* x, void* residual, const void* weight, float eps, int64_t num_tokens,
+                                     int hidden, void* xq, float* scales, sllm_dtype_t dtype, sllm_stream_t stream);
+int sllm_silu_and_mul_quant_fp8(const void* x, int64_t x_row_stride, int64_t num_tokens, int64_t F, void* out, float* scales,
+                                sllm_dtype_t dtype, sllm_stream_t stream);
+int sllm_quant_fp8_rows(const void* x, int64_t x_row_stride, int64_t num_rows, int64_t cols, void* out, float* scales,
+                        sllm_dtype_t dtype, sllm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -58,6 +58,9 @@ SIGNATURES = {
     "sllm_constrain_logits": (_I, [_P, _L, _I, _L, _L, _P, _P, _L, _I, _P, _P, _L, _P, _P, _L, _I, _P]),
     "sllm_lora_shrink": (_I, [_P, _L, _L, _I, _P, _L, _P, _L, _I, _P, _L, _P, _I, _I, _P]),
     "sllm_lora_expand": (_I, [_P, _L, _L, _I, _P, _L, _P, _L, _I, _I, _I, _P, _L, _P, _P, _I, _I, _P]),
+    "sllm_fused_add_rmsnorm_quant_fp8": (_I, [_P, _P, _P, _F, _L, _I, _P, _P, _I, _P]),
+    "sllm_silu_and_mul_quant_fp8": (_I, [_P, _L, _L, _L, _P, _P, _I, _P]),
+    "sllm_quant_fp8_rows": (_I, [_P, _L, _L, _L, _P, _P, _I, _P]),
 }
 
 _lib = None

@@ -59,6 +59,10 @@ class EngineConfig:
     # their largest rank, one of 8, 16, 32, 64 (storage padded to a multiple of 16).  max_loras 0: nothing is allocated
     max_loras: int = 0
     max_lora_rank: int = 0
+    # FP8 (e4m3) projection weights (worker/fp8.py): None follows the checkpoint (a supported FP8 quantization_config turns FP8 on,
+    # none is the 16-bit engine); "fp8" also quantizes 16-bit weights at load.  Activations, norms, embeddings, lm_head and the KV
+    # cache stay 16-bit; activations are quantized per token at run time.  Needs dtype "bfloat16"
+    quantization: object = None
 
     @staticmethod
     def add_cli_args(parser: argparse.ArgumentParser):
@@ -75,3 +79,6 @@ class EngineConfig:
         parser.add_argument("--max-tokens-in-batch", type=int, default=32768, help="Maximum number of tokens in a batch")
         parser.add_argument("--dtype", type=str, default="float16", choices=["float16", "bfloat16"])
         parser.add_argument("--use-cuda-graph", action="store_true")
+        parser.add_argument("--quantization", type=str, default=None, choices=["fp8"],
+                            help="fp8: e4m3 projection weights (16-bit checkpoints are quantized at load); default: follow the "
+                                 "checkpoint's quantization_config")

@@ -11,13 +11,19 @@ side stream for decode attention (:103-114) is only used when the batch really m
 Per-request LoRA adapters (infer_state.lora, worker/lora.py): right after each of the four GEMMs (qkv, o, up_gate, down) a
 shrink and an expand launch add the adapters' deltas into the GEMM output in place - under TP into the rank's partial output
 (the NCCL buffer or comm.partial_out) before the exchange sums the ranks.
+
+FP8 weights (weight.fp8, worker/fp8.py): the same sequence with e4m3 GEMM inputs.  The kernels that produce each input quantize it
+per token (csrc/fp8.cu) and the GEMMs are the library's row-wise scaled FP8 GEMM (linear_fp8): add+RMSNorm+quantize -> qkv ->
+rotary / KV store / attention as above -> quantize -> o_proj -> add+RMSNorm+quantize (or the exchange, then quantize) -> up_gate
+-> SiLU*mul+quantize -> down_proj.  Under TP the row-parallel inputs are quantized per rank on the rank's K slice.
 """
 import torch
 import torch.distributed as dist
 
 from swiftllm_b200.worker.infer_state import LlamaInferState
 from swiftllm_b200.worker.kernels.kvcache_mgmt import rotary_store_kvcache_decode, store_kvcache
-from swiftllm_b200.worker.kernels.linear import linear
+from swiftllm_b200.worker.kernels.fp8 import fused_add_rmsnorm_quant_fp8, quant_fp8_rows, silu_and_mul_quant_fp8
+from swiftllm_b200.worker.kernels.linear import linear, linear_fp8
 from swiftllm_b200.worker.kernels.lora import lora_expand, lora_shrink
 from swiftllm_b200.worker.kernels.paged_attn import paged_attention
 from swiftllm_b200.worker.kernels.prefill_attn import paged_attention_verify, prefill_attention, prefill_attention_paged
@@ -55,29 +61,11 @@ class LlamaTransformerLayer:
         lora_shrink(x, p.u, p.a[self.layer_id][site], lora.tiles, mask)
         lora_expand(y, p.u, p.b[self.layer_id][site], p.dims_ends[site], lora.tiles, mask, p.scales)
 
-    def forward(
-        self,
-        input_embds: torch.Tensor,  # [num_tokens, hidden_size]
-        residual_buf: torch.Tensor,  # [num_tokens, hidden_size]
-        k_cache: torch.Tensor,
-        v_cache: torch.Tensor,
-        block_table: torch.Tensor,
-        infer_state: LlamaInferState,
-    ) -> torch.Tensor:
-        mc, w = self.model_config, self.weight
-        # fused exchange (tp_comm.py) for steps it covers; the same choice in every layer of a step (the row count is fixed)
-        comm = self.comm if (self.comm is not None and residual_buf.shape[0] <= self.comm.max_fused_tokens) else None
-        if comm is not None and self.layer_id > 0:
-            # the previous layer left its down_proj PARTIAL in symmetric buffer 1: exchange + add + norm in one kernel
-            input_embds = comm.reduce_add_norm(1, residual_buf.shape[0], residual_buf, w.attn_norm, mc.rms_norm_eps)
-        else:
-            fused_add_rmsnorm_inplace(input_embds, residual_buf, w.attn_norm, mc.rms_norm_eps)
-
-        # one GEMM for q, k and v (three latency-bound GEMMs in the reference, transformer_layer.py:54-56); the
-        # kernels below take the row-strided column slices directly
-        qkv = linear(input_embds, w.qkv_proj)
-        lora = infer_state.lora
-        self._lora(lora, 0, input_embds, qkv)
+    def _attention(self, qkv: torch.Tensor, input_embds: torch.Tensor, k_cache, v_cache, block_table,
+                   infer_state: LlamaInferState) -> torch.Tensor:
+        """Rotary, KV store and attention of the qkv GEMM output; the attention output [T, nq * D] (at TP 1 written over
+        input_embds, which the GEMM has consumed)."""
+        mc = self.model_config
         T, nqd, nkvd = qkv.shape[0], self.num_q_heads * mc.head_dim, self.num_kv_heads * mc.head_dim
         q = qkv[:, :nqd].unflatten(1, (self.num_q_heads, mc.head_dim))
         k = qkv[:, nqd:nqd + nkvd].unflatten(1, (self.num_kv_heads, mc.head_dim))
@@ -120,6 +108,34 @@ class LlamaTransformerLayer:
             else:
                 paged_attention(q[npt:], k_cache, v_cache, block_table, mc, self.engine_config, infer_state,
                                 self.layer_id, o[npt:])
+        return o
+
+    def forward(
+        self,
+        input_embds: torch.Tensor,  # [num_tokens, hidden_size]
+        residual_buf: torch.Tensor,  # [num_tokens, hidden_size]
+        k_cache: torch.Tensor,
+        v_cache: torch.Tensor,
+        block_table: torch.Tensor,
+        infer_state: LlamaInferState,
+    ) -> torch.Tensor:
+        mc, w = self.model_config, self.weight
+        # fused exchange (tp_comm.py) for steps it covers; the same choice in every layer of a step (the row count is fixed)
+        comm = self.comm if (self.comm is not None and residual_buf.shape[0] <= self.comm.max_fused_tokens) else None
+        if w.fp8:
+            return self._forward_fp8(input_embds, residual_buf, k_cache, v_cache, block_table, infer_state, comm)
+        if comm is not None and self.layer_id > 0:
+            # the previous layer left its down_proj PARTIAL in symmetric buffer 1: exchange + add + norm in one kernel
+            input_embds = comm.reduce_add_norm(1, residual_buf.shape[0], residual_buf, w.attn_norm, mc.rms_norm_eps)
+        else:
+            fused_add_rmsnorm_inplace(input_embds, residual_buf, w.attn_norm, mc.rms_norm_eps)
+
+        # one GEMM for q, k and v (three latency-bound GEMMs in the reference, transformer_layer.py:54-56); the
+        # kernels below take the row-strided column slices directly
+        qkv = linear(input_embds, w.qkv_proj)
+        lora = infer_state.lora
+        self._lora(lora, 0, input_embds, qkv)
+        o = self._attention(qkv, input_embds, k_cache, v_cache, block_table, infer_state)
 
         if comm is not None:
             T = o.shape[0]
@@ -146,4 +162,28 @@ class LlamaTransformerLayer:
         ffn_out = linear(up_gate_proj[:, :self.ffn_inter_dim], w.down_proj)
         self._lora(lora, 3, up_gate_proj[:, :self.ffn_inter_dim], ffn_out)
         self._all_reduce(ffn_out)
+        return ffn_out
+
+    def _forward_fp8(self, input_embds, residual_buf, k_cache, v_cache, block_table, infer_state, comm):
+        mc, w, dt = self.model_config, self.weight, residual_buf.dtype
+        if comm is not None and self.layer_id > 0:
+            xq, xs = quant_fp8_rows(comm.reduce_add_norm(1, residual_buf.shape[0], residual_buf, w.attn_norm, mc.rms_norm_eps))
+        else:
+            xq, xs = fused_add_rmsnorm_quant_fp8(input_embds, residual_buf, w.attn_norm, mc.rms_norm_eps)
+        qkv = linear_fp8(xq, xs, w.qkv_proj, w.qkv_proj_scale, dt)
+        o = self._attention(qkv, input_embds, k_cache, v_cache, block_table, infer_state)
+        oq, os_ = quant_fp8_rows(o)
+        T = o.shape[0]
+        if comm is not None:
+            linear_fp8(oq, os_, w.o_proj, w.o_proj_scale, dt, out=comm.partial_out(0, T))   # partial sums -> symmetric buffer 0
+            xq, xs = quant_fp8_rows(comm.reduce_add_norm(0, T, residual_buf, w.ffn_norm, mc.rms_norm_eps))
+        else:
+            o = linear_fp8(oq, os_, w.o_proj, w.o_proj_scale, dt)                          # row-parallel under TP: partial sums
+            self._all_reduce(o)
+            xq, xs = fused_add_rmsnorm_quant_fp8(o, residual_buf, w.ffn_norm, mc.rms_norm_eps)
+        up_gate_proj = linear_fp8(xq, xs, w.up_gate_proj, w.up_gate_proj_scale, dt)
+        hq, hs = silu_and_mul_quant_fp8(up_gate_proj)
+        ffn_out = linear_fp8(hq, hs, w.down_proj, w.down_proj_scale, dt, out=None if comm is None else comm.partial_out(1, T))
+        if comm is None:
+            self._all_reduce(ffn_out)
         return ffn_out

@@ -37,6 +37,7 @@ from swiftllm_b200.model_config import LlamaModelConfig
 from swiftllm_b200.sampling_params import (ConstraintWords, PromptLogprobs, SamplingParams, TokenLogprobs, constraint_words,
                                            has_penalties, logprobs_top_n, prompt_logprobs_top_n, sampling_words)
 from swiftllm_b200.utils import GB
+from swiftllm_b200.worker import fp8 as fp8_weights
 from swiftllm_b200.worker.block_manager import BlockManager
 from swiftllm_b200.worker.kernels.block_mgmt import copy_block_tails
 from swiftllm_b200.worker.lora import LoraPool, lora_tiles
@@ -100,6 +101,9 @@ class LlamaModel:
         mc = self.model_config
         assert mc.num_q_heads % self.tp_size == 0 and mc.num_kv_heads % self.tp_size == 0 and \
             mc.ffn_inter_dim % self.tp_size == 0, "tp_size must divide q heads, kv heads and ffn_inter_dim"
+        # FP8 projections (worker/fp8.py): unsupported formats and combinations raise ValueError before anything is allocated
+        self.fp8 = fp8_weights.resolve(getattr(engine_config, "quantization", None), mc, self.tp_size,
+                                       getattr(engine_config, "max_loras", 0), self.dtype)
         self.device = torch.device("cuda", torch.cuda.current_device())
 
         self.weight = None
@@ -136,7 +140,7 @@ class LlamaModel:
         self.weight = load_weights(self.model_config, self.dtype, self.engine_config.model_path,
                                    self.engine_config.use_dummy, getter=weight_getter,
                                    tp_rank=self.tp_rank, tp_size=self.tp_size, device=self.device,
-                                   shard_lm_head=self._shard_lm_head())
+                                   shard_lm_head=self._shard_lm_head(), fp8=self.fp8)
         cos, sin = build_rope_tables(self.model_config, self.dtype)
         self._cos_cached, self._sin_cached = cos.to(self.device), sin.to(self.device)
 

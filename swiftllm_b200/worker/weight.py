@@ -18,6 +18,7 @@ from typing import Callable, Optional
 import torch
 
 from swiftllm_b200.model_config import LlamaModelConfig
+from swiftllm_b200.worker import fp8 as fp8_weights
 
 # (attribute, HF key template, shape fn, TP split axis: 0 rows, 1 cols, None replicated)
 _LAYER_ITEMS = [
@@ -47,12 +48,19 @@ class LlamaTransformerLayerWeight:
         self.layer_id = layer_id
         self.model_config = model_config
         self.dtype = dtype
+        self.fp8 = False
 
-    def load_weights(self, getter: Callable, tp_rank: int, tp_size: int, device):
+    def load_weights(self, getter: Callable, tp_rank: int, tp_size: int, device, fp8: bool = False):
+        """fp8: every projection becomes an e4m3 weight plus an fp32 per-output-channel `<name>_scale` (worker/fp8.py)."""
+        if fp8:
+            return self._load_fp8(getter, tp_rank, tp_size, device)
         for attr, key, shape_fn, axis in _LAYER_ITEMS:
             key = key.format(i=self.layer_id)
             shape = shape_fn(self.model_config)
             w = getter(key, shape, self.dtype)
+            if isinstance(w, torch.Tensor) and w.dtype == torch.float8_e4m3fn:
+                raise ValueError(f"{key} is float8_e4m3fn: serve FP8 checkpoints with their quantization_config in config.json "
+                                 f"or EngineConfig.quantization='fp8'")
             assert isinstance(w, torch.Tensor), f"Weight {key} is not a tensor"
             assert tuple(w.shape) == tuple(shape), f"Shape of weight {key} does not match"
             w = tp_slice(w, axis, tp_rank, tp_size).to(device=device, dtype=self.dtype).contiguous()
@@ -68,6 +76,29 @@ class LlamaTransformerLayerWeight:
         self.k_proj = self.qkv_proj[nq_rows:nq_rows + nkv_rows]
         self.v_proj = self.qkv_proj[nq_rows + nkv_rows:]
 
+    def _load_fp8(self, getter: Callable, tp_rank: int, tp_size: int, device):
+        self.fp8 = True
+        for attr, key, shape_fn, axis in _LAYER_ITEMS:
+            key = key.format(i=self.layer_id)
+            shape = shape_fn(self.model_config)
+            if attr in fp8_weights.PROJECTIONS:
+                w, s = fp8_weights.load_projection(getter, key, shape, axis, tp_rank, tp_size, self.dtype, device)
+                setattr(self, attr + "_scale", s)
+            else:
+                w = getter(key, shape, self.dtype)
+                assert isinstance(w, torch.Tensor), f"Weight {key} is not a tensor"
+                assert tuple(w.shape) == tuple(shape), f"Shape of weight {key} does not match"
+                w = tp_slice(w, axis, tp_rank, tp_size).to(device=device, dtype=self.dtype).contiguous()
+            setattr(self, attr, w)
+        # the 16-bit path's fusions, weights and scales concatenated in the same order
+        self.up_gate_proj = fp8_weights.cat_rows((self.up_proj, self.gate_proj))
+        self.up_gate_proj_scale = torch.cat((self.up_proj_scale, self.gate_proj_scale))
+        self.qkv_proj = fp8_weights.cat_rows((self.q_proj, self.k_proj, self.v_proj))
+        self.qkv_proj_scale = torch.cat((self.q_proj_scale, self.k_proj_scale, self.v_proj_scale))
+        for n in ("up_proj", "gate_proj", "q_proj", "k_proj", "v_proj"):
+            delattr(self, n)
+            delattr(self, n + "_scale")
+
 
 class LlamaWeight:
     def __init__(self, model_config: LlamaModelConfig, dtype: torch.dtype, model_version: str = "llama"):
@@ -76,8 +107,11 @@ class LlamaWeight:
         self.model_version = model_version
         self.layers = [LlamaTransformerLayerWeight(i, model_config, dtype) for i in range(model_config.num_layers)]
 
-    def load_weights(self, getter: Callable, tp_rank: int = 0, tp_size: int = 1, device="cuda", shard_lm_head: bool = False):
+    def load_weights(self, getter: Callable, tp_rank: int = 0, tp_size: int = 1, device="cuda", shard_lm_head: bool = False,
+                     fp8: bool = False):
         c = self.model_config
+        if fp8:
+            fp8_weights.check_no_static_activation_scales(getter)
         vs = (c.vocab_size, c.hidden_size)
         self.wte = getter("model.embed_tokens.weight", vs, self.dtype).to(device=device, dtype=self.dtype)
         self.lm_head_sharded = bool(shard_lm_head) and tp_size > 1
@@ -92,7 +126,7 @@ class LlamaWeight:
             self.lm_head = lm_head.to(device=device, dtype=self.dtype).contiguous()
         self.final_norm = getter("model.norm.weight", (c.hidden_size,), self.dtype).to(device=device, dtype=self.dtype)
         for layer in self.layers:
-            layer.load_weights(getter, tp_rank, tp_size, device)
+            layer.load_weights(getter, tp_rank, tp_size, device, fp8=fp8)
 
 
 # ---------------------------------------------------------------- getters
@@ -121,6 +155,7 @@ def synthetic_getter(seed: int = 0, std: float = 0.02, device="cuda"):
 def dict_getter(tensors: dict):
     def get(key, shape, dtype):
         return tensors[key]
+    get.keys = tensors.keys()
     return get
 
 
@@ -142,6 +177,11 @@ def checkpoint_getter(model_path: str, device="cuda"):
             fname = index[key] if index is not None else st_files[0]
             with safetensors.safe_open(os.path.join(model_path, fname), framework="pt", device=str(device)) as f:
                 return f.get_tensor(key)
+        if index is not None:
+            get.keys = index.keys()
+        else:
+            with safetensors.safe_open(os.path.join(model_path, st_files[0]), framework="pt", device="cpu") as f:
+                get.keys = list(f.keys())
         return get
 
     index_path = os.path.join(model_path, "pytorch_model.bin.index.json")
@@ -167,11 +207,11 @@ def detect_model_version(model_path: Optional[str], model_config: LlamaModelConf
 
 def load_weights(model_config: LlamaModelConfig, dtype: torch.dtype, model_path: Optional[str], use_dummy: bool = False,
                  model_version: str = "auto", getter: Optional[Callable] = None, tp_rank: int = 0, tp_size: int = 1,
-                 device="cuda", shard_lm_head: bool = False) -> LlamaWeight:
+                 device="cuda", shard_lm_head: bool = False, fp8: bool = False) -> LlamaWeight:
     if model_version == "auto":
         model_version = detect_model_version(model_path, model_config)
     if getter is None:
         getter = dummy_getter(device) if use_dummy else checkpoint_getter(model_path, device)
     weight = LlamaWeight(model_config, dtype, model_version)
-    weight.load_weights(getter, tp_rank, tp_size, device, shard_lm_head=shard_lm_head)
+    weight.load_weights(getter, tp_rank, tp_size, device, shard_lm_head=shard_lm_head, fp8=fp8)
     return weight
