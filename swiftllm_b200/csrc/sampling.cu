@@ -8,6 +8,9 @@
 //   draw     u = ((x >> 9) + 0.5) * 2^-23 with x = Philox4x32-10(key (seed_lo, seed_hi), counter (v >> 2, pos, 0, 0)) word v & 3,
 //            v the GLOBAL vocabulary index; score = l / T - log(-log u) (fp32, IEEE division, logf); the token is the kept
 //            index with the largest score, smallest index on ties.
+//   NaN / +inf  a row holding a NaN of either sign or +inf, or whose largest logit is -inf, is drawn greedily whatever T, k and
+//            p: the largest key, smallest index among equal ones (a +NaN, else the first +inf, else the argmax of the rest; index
+//            0 of an all -inf row).  Its masses and scores are undefined, so this keeps the token a valid id of the row.
 // Both thresholds are exact: keys are 16 bits, so a radix select over the high and then the low byte finds them.  Masses are
 // summed as 64-bit fixed-point integers (q * 2^40, rounded), so every sum is exact and independent of the order of additions:
 // the result is a pure function of (logits, T, k, p, seed, pos), whatever the cluster size, batch or launch mode.
@@ -57,6 +60,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     __shared__ unsigned long long h_cnt_hi[256], h_cnt_lo[256], h_mass_hi[256], h_mass_lo[256], merged[256];
     __shared__ unsigned long long scratch[32];
     __shared__ unsigned long long cta_max;
+    __shared__ int cta_bad;
     __shared__ float cta_score, warp_score[32];
     __shared__ int64_t cta_index, warp_index[32];
     __shared__ int sel_bin;
@@ -72,23 +76,27 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     // ---- stage the slice as keys; local (max key, smallest index)
     for (int i = threadIdx.x; i < 256; i += blockDim.x) h_cnt_hi[i] = h_cnt_lo[i] = h_mass_hi[i] = h_mass_lo[i] = 0;
     unsigned long long best = 0;
+    bool bad = false;                                                 // a NaN of either sign or +inf
     stage_keys(reinterpret_cast<const uint16_t*>(src), n, keys, [&](uint32_t k, int i) {
         const unsigned long long c = pair_of(k, begin + i);
         best = c > best ? c : best;
+        bad |= k >= InfKeys<T>::pos || k < InfKeys<T>::neg;
     });
     best = block_max_u64(best, scratch);
-    if (threadIdx.x == 0) cta_max = best;
+    bad = __syncthreads_or(bad);
+    if (threadIdx.x == 0) { cta_max = best; cta_bad = bad; }
     cluster.sync();
     unsigned long long gmax = 0;
     for (unsigned r = 0; r < C; r++) {
         const unsigned long long c = *cluster.map_shared_rank(&cta_max, r);
         gmax = c > gmax ? c : gmax;
+        bad |= *cluster.map_shared_rank(&cta_bad, r) != 0;
     }
     const uint32_t max_key = (uint32_t)(gmax >> 32);
     const int64_t max_index = vocab_offset + (int64_t)(0xffffffffu - (uint32_t)gmax);
 
     const float temp = temperature[row];
-    if (!(temp > 0.f)) {                                              // greedy (every CTA of the cluster takes this branch)
+    if (!(temp > 0.f) || bad || max_key <= InfKeys<T>::neg) {        // greedy (every CTA of the cluster takes this branch)
         if (rank == 0 && threadIdx.x == 0) {
             out_tokens[row] = max_index;
             if (out_pairs) { out_pairs[2 * row] = value_of<T>(max_key); out_pairs[2 * row + 1] = (float)max_index; }

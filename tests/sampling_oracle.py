@@ -7,6 +7,8 @@
              from the top is >= p * sum(q);
     draw     x = Philox4x32-10(key (seed_lo, seed_hi), counter (v >> 2, pos, 0, 0)) word v & 3, u = ((x >> 9) + 0.5) * 2^-23,
              score = fp32(l) / T + (-log(-log u)) in fp32, token = first index of the largest score among the kept tokens.
+    bad rows a NaN of either sign or +inf anywhere, or a largest logit of -inf: drawn greedily whatever T, k and p (the first
+             index of the largest key: a +NaN, else the first +inf, else the argmax of the rest).
 The kernel sums masses in 2^-40 fixed point and uses CUDA's logf, so the tests exempt rows whose top-p boundary or top-2 score
 gap is within rounding of those differences (`boundary_margin`, `gap`)."""
 from __future__ import annotations
@@ -59,7 +61,9 @@ def sample_row(bits: np.ndarray, vals: np.ndarray, temperature, top_k, top_p, se
     V = bits.shape[0]
     keys = keys_of(bits)
     T = np.float32(temperature)
-    if not T > 0:
+    with np.errstate(invalid="ignore"):
+        bad = bool(np.isnan(vals).any() or np.isposinf(vals).any() or not (vals > -np.inf).any())
+    if not T > 0 or bad:
         i = int(np.argmax(keys))
         return RowResult(vocab_offset + i, float(vals[i]), None, np.inf, np.inf)
     kept = np.ones(V, dtype=bool)
