@@ -89,7 +89,8 @@ static int launch_rmsnorm(void* x, void* residual, const void* weight, float eps
     }
     const int threads = row_threads(nvec);
     size_t smem = (size_t)nvec * sizeof(uint4);
-    if (smem > 48 * 1024)
+    // the 48 KB a kernel may use without raising its limit include its static shared memory: red[16]
+    if (smem + 16 * sizeof(float) > 48 * 1024)
         cudaFuncSetAttribute(rmsnorm_kernel<T, FUSED, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     rmsnorm_kernel<T, FUSED, 0><<<(unsigned)T_, threads, smem, stream>>>((T*)x, (T*)residual, (const T*)weight, eps, hidden);
     return check_launch(what);

@@ -192,7 +192,8 @@ int launch_add_rmsnorm_quant(const void* x, void* residual, const void* weight, 
         return check_launch("fused_add_rmsnorm_quant_fp8");
     }
     const size_t smem = (size_t)nvec * sizeof(uint4);
-    if (smem > 48 * 1024)
+    // the 48 KB a kernel may use without raising its limit include its static shared memory: red[16], redmax[16]
+    if (smem + 32 * sizeof(float) > 48 * 1024)
         cudaFuncSetAttribute(add_rmsnorm_quant_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     add_rmsnorm_quant_kernel<T, 0><<<(unsigned)T_, row_threads(nvec), smem, stream>>>((const T*)x, (T*)residual, (const T*)weight,
                                                                                       eps, hidden, (uint8_t*)xq, scales);
@@ -235,7 +236,7 @@ int sllm_silu_and_mul_quant_fp8(const void* x, int64_t x_row_stride, int64_t num
     const int nvec = (int)(F / 8);
     const size_t smem = (size_t)nvec * sizeof(uint4);
     SLLM_DISPATCH_DTYPE(dtype, {
-        if (smem > 48 * 1024)
+        if (smem + 16 * sizeof(float) > 48 * 1024)     // static shared memory (redmax[16]) counts against the 48 KB
             cudaFuncSetAttribute(silu_and_mul_quant_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         silu_and_mul_quant_kernel<T><<<(unsigned)num_tokens, row_threads(nvec), smem, (cudaStream_t)stream>>>(
             (const T*)x, x_row_stride, (int)F, (uint8_t*)out, scales);

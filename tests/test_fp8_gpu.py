@@ -39,7 +39,7 @@ def _check(q, s, ref_q, ref_s):
 
 # ---------------------------------------------------------------- kernels
 @pytest.mark.parametrize("dt", DTYPES, ids=["fp16", "bf16"])
-@pytest.mark.parametrize("H", [4096, 8192, 2048, 1024, 1040])        # 1024: the 2-vectors-per-thread instance
+@pytest.mark.parametrize("H", [4096, 8192, 2048, 3072, 1024, 3584, 1040, 24576, 28672])  # 1024, 3584: VPT = 2; 24576 up: > 48 KB
 @pytest.mark.parametrize("T", [1, 7, 64, 997])
 @pytest.mark.parametrize("kind", ["normal", "outliers", "subnormal"])
 def test_add_rmsnorm_quant_bit_for_bit(dt, H, T, kind):
@@ -60,7 +60,7 @@ def test_add_rmsnorm_quant_bit_for_bit(dt, H, T, kind):
 
 
 @pytest.mark.parametrize("dt", DTYPES, ids=["fp16", "bf16"])
-@pytest.mark.parametrize("F", [14336, 7168, 1792, 208])
+@pytest.mark.parametrize("F", [14336, 7168, 1792, 208, 24576, 28672])  # 24576 up: > 48 KB of shared memory
 @pytest.mark.parametrize("T", [1, 64, 601])
 @pytest.mark.parametrize("kind", ["normal", "outliers", "subnormal"])
 def test_silu_and_mul_quant_bit_for_bit(dt, F, T, kind):
