@@ -17,7 +17,8 @@ whose count it can change, so its host cost does not grow with the number of oth
 import numpy as np
 import torch
 
-from .kernels.block_mgmt import (allocate_blocks_for_seqs as _allocate_kernel,
+from .kernels.block_mgmt import (MAX_ALLOCATE_BATCH,
+                                 allocate_blocks_for_seqs as _allocate_kernel,
                                  fork_blocks_for_seqs as _fork_kernel,
                                  gather_allocated_blocks_and_unset,
                                  release_blocks_for_seqs as _release_kernel,
@@ -71,8 +72,12 @@ class BlockManager:
 
     def reserve_blocks_for_seqs(self, seq_ids_list, target_lens_list) -> int:
         """Host half of allocate_blocks_for_seqs: count ceil(target_lens_list[i] / block_size) blocks for seq #i into the host
-        mirror and `num_free_blocks`, and return how many are new.  Raises RuntimeError, changing nothing, when a sequence would
-        need more than max_blocks_per_seq blocks or the free blocks do not suffice; the caller then enqueues nothing."""
+        mirror and `num_free_blocks`, and return how many are new.  Raises RuntimeError, changing nothing, when the batch is larger
+        than the allocation kernel takes, a sequence would need more than max_blocks_per_seq blocks or the free blocks do not
+        suffice; the caller then enqueues nothing."""
+        if len(seq_ids_list) > MAX_ALLOCATE_BATCH:
+            raise RuntimeError(f"cannot allocate blocks for {len(seq_ids_list)} sequences in one call "
+                               f"(at most {MAX_ALLOCATE_BATCH})")
         idx = np.asarray(seq_ids_list, dtype=np.int64)
         target = (np.asarray(target_lens_list, dtype=np.int64) + (self.block_size - 1)) // self.block_size
         have = self._host_nsab[idx]
@@ -102,6 +107,8 @@ class BlockManager:
         validated the lists (empty, distinct dst rows that are no src; 1 <= lens[i] <= blocks held by src * block_size) and copies
         the tail pages.  Raises RuntimeError, before any device work, when the tail blocks do not fit."""
         bs = self.block_size
+        if len(dst_seq_ids_list) > MAX_ALLOCATE_BATCH:
+            raise RuntimeError(f"cannot fork {len(dst_seq_ids_list)} sequences in one call (at most {MAX_ALLOCATE_BATCH})")
         tails = sum(1 for p in lens_list if p % bs)
         if tails > self.num_free_blocks:
             raise RuntimeError(f"No enough free blocks available on {self.device_name} ({self.num_blocks} in total, "

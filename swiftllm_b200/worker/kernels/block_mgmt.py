@@ -4,6 +4,9 @@ import torch
 
 from swiftllm_b200 import _lib
 
+# Largest batch sllm_allocate_blocks_for_seqs takes: its kernel keeps 2 * batch + 1 int32 in at most 200 KB of shared memory.
+MAX_ALLOCATE_BATCH = (200 * 1024 // 4 - 1) // 2
+
 
 def set_block_table_and_num_seq_alloc_blocks(
     num_seq_allocated_blocks: torch.Tensor,  # [max_seqs_in_block_table]

@@ -28,6 +28,21 @@ def allocate(nsab, table, is_free, seq_ids, lens, bs):
     return out
 
 
+def allocate_status(nsab, is_free, seq_ids, lens, bs, mbps, cap=None):
+    """The allocation kernel's status word [new blocks or 0, flags] for a call given these inputs.  Flags: 2 a sequence holds more
+    blocks than its target, 4 a target above mbps, 1 too few free blocks (checked only without flag 2 or 4), 8 more new blocks
+    than `cap` (the length of new_out, when one is given).  With any flag set the kernel changes nothing."""
+    have = np.asarray([int(nsab[s]) for s in seq_ids], dtype=np.int64)
+    tgt = (np.asarray(lens, dtype=np.int64) + bs - 1) // bs
+    err = (2 if (have > tgt).any() else 0) | (4 if (tgt > mbps).any() else 0)
+    total = int(np.maximum(tgt - have, 0).sum())
+    if err == 0 and total > 0 and int(np.count_nonzero(is_free)) < total:
+        err |= 1
+    if cap is not None and total > cap:
+        err |= 8
+    return [0 if err else total, err]
+
+
 def fork_rows(nsab, table, extra, src_ids, dst_ids, lens, bs):
     """The fork kernel alone: shares the leading blocks; the tail block comes from `allocate`."""
     for s, d, p in zip(src_ids, dst_ids, lens):

@@ -29,12 +29,15 @@ AHEAD = 1000            # flags pre-filled with epoch + AHEAD: a peer that is "a
 EXTRA_ROWS = 3          # rows past the T in use in x_out / residual: a kernel must leave them alone
 
 # (N, H, T).  H = 8: 1 vector / 32 threads;  1032: 129 vectors, 160 threads (ragged loop);  4096: 512 threads;  8192: two
-# vectors per thread;  28672: 56 KB of dynamic shared memory (the cudaFuncSetAttribute path; the LL kernel refuses it).
+# vectors per thread;  24544 / 24552 / 24576: the 48 KB edge, where the row plus the kernel's static shared memory (64 B, two-shot
+# 80 B) first needs the raised limit;  28672: 56 KB of dynamic shared memory (the LL kernel refuses it).  The raised limit lasts
+# for the process, so the edge cases come before the 28672 ones: after 28672 they would pass without testing the launcher.
 # T = N - 1 leaves a rank without a row to own;  T = None stands for 2 * SMs + 5 (LL: CTAs loop over several rows);
 # T = 1024 is the largest LL exchange (MAX_LL_TOKENS).
 FLAG_CASES = [(2, 8, 1), (8, 4096, 1), (3, 1032, 2), (4, 4096, 5), (8, 8192, 7), (8, 1032, 131), (2, 4096, 131),
-              (3, 8192, 131), (3, 28672, 4), (4, 28672, 3), (8, 28672, 9), (4, 8192, 1024), (2, 1032, 1024), (8, 8, 1024)]
-LL_CASES = [(2, 8, 1), (8, 4096, 1), (3, 1032, 2), (4, 4096, 5), (8, 8192, 7), (8, 1032, 131), (2, 8, 131), (2, 4096, None),
+              (3, 8192, 131), (2, 24544, 3), (3, 24552, 2), (4, 24576, 5), (3, 28672, 4), (4, 28672, 3), (8, 28672, 9), (4, 8192, 1024), (2, 1032, 1024), (8, 8, 1024)]
+LL_CASES = [(2, 8, 1), (8, 4096, 1), (3, 1032, 2), (4, 4096, 5), (8, 8192, 7), (8, 1032, 131), (2, 8, 131), (2, 24544, 3),
+            (3, 24552, 2), (4, 24576, 5), (2, 4096, None),
             (4, 1032, None), (8, 8192, None), (4, 8192, 1024), (3, 4096, 1024), (8, 8, 1024)]
 
 
@@ -278,16 +281,18 @@ def test_ll_vs_restatement_and_two_shot(case, dtype):
 
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_ll_rejects_a_row_too_large_for_shared_memory(dtype):
-    L, N, H, T = _lib(), 2, 28672, 2
-    x = torch.zeros(T, H, dtype=dtype, device=DEV)
-    st = torch.zeros(32, dtype=torch.int32, device=DEV)
-    bufs = _ptrs([x, x])
-    rc = L.lib().sllm_allreduce_add_rmsnorm_ll(x.data_ptr(), ctypes.cast(bufs, ctypes.c_void_p), ctypes.cast(bufs, ctypes.c_void_p),
-                                               None, 0, N, 0, st.data_ptr(), x.data_ptr(), x.data_ptr(), x[0].data_ptr(), EPS, T, H,
-                                               1, L.dtype_tag(dtype), L.stream())
-    assert rc != 0 and b"too large" in L.lib().sllm_last_error()
-    torch.cuda.synchronize()
-    assert int(st.abs().sum()) == 0
+    """24584 is the first width past the 48 KB row the LL check accepts (LL_CASES runs 24576); 28672 is a model's."""
+    L, N, T = _lib(), 2, 2
+    for H in (24584, 28672):
+        x = torch.zeros(T, H, dtype=dtype, device=DEV)
+        st = torch.zeros(32, dtype=torch.int32, device=DEV)
+        bufs = _ptrs([x, x])
+        rc = L.lib().sllm_allreduce_add_rmsnorm_ll(x.data_ptr(), ctypes.cast(bufs, ctypes.c_void_p), ctypes.cast(bufs, ctypes.c_void_p),
+                                                   None, 0, N, 0, st.data_ptr(), x.data_ptr(), x.data_ptr(), x[0].data_ptr(), EPS, T,
+                                                   H, 1, L.dtype_tag(dtype), L.stream())
+        assert rc != 0 and b"too large" in L.lib().sllm_last_error(), H
+        torch.cuda.synchronize()
+        assert int(st.abs().sum()) == 0 and int(x.abs().sum()) == 0, H
 
 
 # ----------------------------------------------------------------------------- epochs
