@@ -190,8 +190,9 @@ extern "C" int sllm_allreduce_add_rmsnorm_ll(const void* partial, void* const* h
     const int64_t cap = 2LL * num_sms();                             // one wave below 512 threads, two at 512: see the kernel comment
     const unsigned grid = (unsigned)(num_tokens < cap ? num_tokens : cap);
     const bool nvls = mc_ag_recv != nullptr;
-    return launch_exchange("allreduce(LL)", "allreduce_add_rmsnorm_ll",
-                           nvls ? allreduce_add_rmsnorm_ll_kernel<__half, true> : allreduce_add_rmsnorm_ll_kernel<__half, false>,
-                           nvls ? allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, true> : allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, false>,
-                           dtype, grid, hidden, (cudaStream_t)stream, p);
+    const char* who = "allreduce(LL)", *kernel = "allreduce_add_rmsnorm_ll";
+    return nvls ? launch_exchange<allreduce_add_rmsnorm_ll_kernel<__half, true>, allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, true>>(
+                      who, kernel, dtype, grid, hidden, (cudaStream_t)stream, p)
+                : launch_exchange<allreduce_add_rmsnorm_ll_kernel<__half, false>, allreduce_add_rmsnorm_ll_kernel<__nv_bfloat16, false>>(
+                      who, kernel, dtype, grid, hidden, (cudaStream_t)stream, p);
 }

@@ -204,10 +204,11 @@ extern "C" int sllm_allreduce_add_rmsnorm_2shot(const void* const* host_peer_buf
     p.mc_buf = mc_buf; p.mc_xout = mc_xout;
     const bool nvls = mc_buf != nullptr;
     const unsigned grid = (unsigned)((num_tokens + nranks - 1) / nranks);        // the same on every rank
-    return launch_exchange("allreduce(2-shot)", "allreduce_add_rmsnorm_2shot",
-                           nvls ? allreduce_add_rmsnorm_2shot_kernel<__half, true> : allreduce_add_rmsnorm_2shot_kernel<__half, false>,
-                           nvls ? allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, true> : allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, false>,
-                           dtype, grid, hidden, (cudaStream_t)stream, p);
+    const char* who = "allreduce(2-shot)", *kernel = "allreduce_add_rmsnorm_2shot";
+    return nvls ? launch_exchange<allreduce_add_rmsnorm_2shot_kernel<__half, true>, allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, true>>(
+                      who, kernel, dtype, grid, hidden, (cudaStream_t)stream, p)
+                : launch_exchange<allreduce_add_rmsnorm_2shot_kernel<__half, false>, allreduce_add_rmsnorm_2shot_kernel<__nv_bfloat16, false>>(
+                      who, kernel, dtype, grid, hidden, (cudaStream_t)stream, p);
 }
 
 // host_peer_bufs / host_peer_flags: HOST arrays of `nranks` device pointers (the symmetric buffer and the signal pad of
@@ -223,6 +224,6 @@ extern "C" int sllm_allreduce_add_rmsnorm(const void* const* host_peer_bufs, voi
     for (int r = 0; r < nranks; r++) { p.peer_buf[r] = host_peer_bufs[r]; p.peer_flags[r] = (uint32_t*)host_peer_flags[r]; }
     p.epoch = (uint32_t*)epoch_state; p.x_out = x_out; p.residual = residual; p.weight = weight; p.eps = eps;
     p.rank = rank; p.nranks = nranks; p.hidden = hidden; p.slot = slot; p.has_norm = weight != nullptr;
-    return launch_exchange("allreduce", "allreduce_add_rmsnorm", allreduce_add_rmsnorm_kernel<__half>,
-                           allreduce_add_rmsnorm_kernel<__nv_bfloat16>, dtype, (unsigned)num_tokens, hidden, (cudaStream_t)stream, p);
+    return launch_exchange<allreduce_add_rmsnorm_kernel<__half>, allreduce_add_rmsnorm_kernel<__nv_bfloat16>>(
+        "allreduce", "allreduce_add_rmsnorm", dtype, (unsigned)num_tokens, hidden, (cudaStream_t)stream, p);
 }

@@ -126,6 +126,33 @@ static inline int row_threads(int nvec) {
 
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// ---------------------------------------------------------------- elementwise formulas
+// h(up * h(silu(f(gate)))) of 8 values: silu in fp32 (IEEE division), rounded to the storage dtype before the product
+template <typename T> __device__ __forceinline__ Vec8<T> silu_mul8(const Vec8<T>& up, const Vec8<T>& gate) {
+    using TT = Traits<T>;
+    Vec8<T> o;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        float2 g = TT::to_f2(gate.v[j]);
+        g.x = g.x / (1.0f + expf(-g.x));
+        g.y = g.y / (1.0f + expf(-g.y));
+        o.v[j] = __hmul2_rn(up.v[j], TT::from_f2(g));
+    }
+    return o;
+}
+// Rotary embedding of one 8-wide chunk x0 of a head's first half and its partner x1 in the second half:
+// o0 = x0·c − x1·s, o1 = x0·s + x1·c, every product and sum rounded to the storage dtype (the *_rn intrinsics forbid FMA
+// contraction), as rotary_emb.py:32-41 evaluates under the Triton interpreter.
+template <typename T>
+__device__ __forceinline__ void rotate8(Vec8<T>& o0, Vec8<T>& o1, const Vec8<T>& x0, const Vec8<T>& x1, const Vec8<T>& c,
+                                        const Vec8<T>& s) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        o0.v[j] = __hsub2_rn(__hmul2_rn(x0.v[j], c.v[j]), __hmul2_rn(x1.v[j], s.v[j]));
+        o1.v[j] = __hadd2_rn(__hmul2_rn(x0.v[j], s.v[j]), __hmul2_rn(x1.v[j], c.v[j]));
+    }
+}
+
 // ---------------------------------------------------------------- per-device one-time state (a process may drive several GPUs)
 static inline int current_device() {
     int d = 0;
@@ -133,11 +160,20 @@ static inline int current_device() {
     return d;
 }
 int num_sms();   // multiprocessors of the current device, cached
-// true exactly once per (call site's mask, device): e.g. cudaFuncSetAttribute, which is a per-device setting
-static inline bool first_use_on_this_device(unsigned long long& mask) {
-    const unsigned long long bit = 1ull << (current_device() & 63);
-    const unsigned long long old = __atomic_fetch_or(&mask, bit, __ATOMIC_RELAXED);
-    return (old & bit) == 0;
+
+// ---------------------------------------------------------------- dynamic shared-memory limit
+// A kernel's launches may use 48 KB of shared memory, static and dynamic together; past that the kernel's dynamic shared-memory
+// limit, a per-device attribute, must first be raised.  Every launcher with dynamic shared memory calls
+// fit_dynamic_smem<Kernel>(bytes, its name) before the launch.  `covered` is, per kernel and device, the dynamic size its launches
+// may use as things stand: 0 until the slow path (host.cu) has read the kernel's static size from the compiled kernel, then 48 KB
+// minus that, and after a raise the raised limit.  It only grows, so a launch it covers costs no driver call and no lock.  The
+// slow path must not run under stream capture: the decode graphs' warm-up launches every kernel of their shapes eagerly first.
+int raise_dynamic_smem(const void* kernel, size_t bytes, int& covered, const char* who);
+template <auto Kernel> inline int fit_dynamic_smem(size_t bytes, const char* who) {
+    static int covered[64];
+    int& c = covered[current_device() & 63];
+    if ((int64_t)bytes <= __atomic_load_n(&c, __ATOMIC_RELAXED)) return 0;
+    return raise_dynamic_smem(reinterpret_cast<const void*>(Kernel), bytes, c, who);
 }
 
 // dispatch on the dtype tag

@@ -83,17 +83,14 @@ static inline int check_exchange(const char* who, int rank, int nranks, int slot
     return 0;
 }
 
-// The dtype's instantiation, launched with row_threads threads and one row of dynamic shared memory.  The 48 KB a kernel may use
-// without raising its limit include its static shared memory: red[16] in all three kernels (64 B), plus s_last in the two-shot
-// kernel (80 B as ptxas lays it out).  The launcher counts the larger for all three.
-template <typename P>
-static int launch_exchange(const char* who, const char* kernel, void (*f16)(P), void (*bf16)(P), sllm_dtype_t dtype,
-                           unsigned grid, int hidden, cudaStream_t st, const P& p) {
+// The dtype's instantiation, F16 or BF16, launched with row_threads threads and one row of dynamic shared memory
+template <auto F16, auto BF16, typename P>
+static int launch_exchange(const char* who, const char* kernel, sllm_dtype_t dtype, unsigned grid, int hidden, cudaStream_t st,
+                           const P& p) {
     SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "%s: unknown dtype tag %d", who, (int)dtype);
-    void (*k)(P) = dtype == SLLM_F16 ? f16 : bf16;
     const size_t smem = (size_t)(hidden / 8) * sizeof(uint4);
-    if (smem + 80 > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k<<<grid, row_threads(hidden / 8), smem, st>>>(p);
+    if (int e = dtype == SLLM_F16 ? fit_dynamic_smem<F16>(smem, kernel) : fit_dynamic_smem<BF16>(smem, kernel)) return e;
+    (dtype == SLLM_F16 ? F16 : BF16)<<<grid, row_threads(hidden / 8), smem, st>>>(p);
     return check_launch(kernel);
 }
 

@@ -46,6 +46,29 @@ int num_sms() {
     return sms[dev];
 }
 
+int raise_dynamic_smem(const void* kernel, size_t bytes, int& covered, const char* who) {
+    static std::mutex m;             // two threads raising one kernel's limit: the larger value must be the one that stays
+    std::lock_guard<std::mutex> lk(m);
+    int limit = covered;
+    cudaError_t e = cudaSuccess;
+    if (limit == 0) {
+        cudaFuncAttributes fa;
+        e = cudaFuncGetAttributes(&fa, kernel);
+        limit = 48 * 1024 - (int)fa.sharedSizeBytes;
+    }
+    if (e == cudaSuccess && (int64_t)bytes > limit) {
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        limit = (int)bytes;
+    }
+    if (e != cudaSuccess) {
+        cudaGetLastError();          // reported here, not by the next launch's check_launch
+        set_error("%s: cannot allow %zu bytes of dynamic shared memory: %s", who, bytes, cudaGetErrorString(e));
+        return (int)e;
+    }
+    __atomic_store_n(&covered, limit, __ATOMIC_RELAXED);
+    return 0;
+}
+
 namespace tc {
 // cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda)
 TensorMapEncodeFn get_tensor_map_encoder() {

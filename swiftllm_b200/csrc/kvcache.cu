@@ -456,10 +456,7 @@ int sllm_allocate_blocks_for_seqs(int32_t* nsab, int32_t* block_table, uint8_t* 
     SLLM_REQUIRE(batch == 0 || (nsab && block_table && is_free && seq_ids && target_lens), "allocate_blocks: null pointer");
     const size_t smem = (size_t)(2 * batch + 1) * sizeof(int32_t);
     SLLM_REQUIRE(smem <= 200 * 1024, "allocate_blocks: batch %d too large", batch);
-    // the 48 KB a kernel may use without raising its limit include its static shared memory: warp_sums[32] and s_err, 144 B as
-    // ptxas lays them out
-    if (smem + 144 > 48 * 1024)
-        cudaFuncSetAttribute(allocate_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (int e = fit_dynamic_smem<allocate_blocks_kernel>(smem, "allocate_blocks_for_seqs")) return e;
     allocate_blocks_kernel<<<1, 1024, smem, (cudaStream_t)stream>>>(nsab, block_table, is_free, seq_ids, target_lens, batch,
                                                                    block_size, num_blocks, mbps, new_out, cap, status);
     return check_launch("allocate_blocks_for_seqs");

@@ -277,10 +277,8 @@ static int choose_split_tokens(int num_seqs, int nkv, int max_seq_len, int seq_b
 template <typename T, int D>
 static int launch_paged(const PagedAttnParams& p, int num_seqs, int max_seq_len, cudaStream_t stream) {
     const size_t smem = (size_t)PA_STAGES * 2 * PA_TILE * D * 2 + (size_t)(p.split_tokens / p.block_size + 2) * sizeof(int32_t);
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(paged_attn_kernel<T, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
     SLLM_REQUIRE(smem <= 110 * 1024, "paged_attention: split too long for shared memory (%zu bytes)", smem);
+    if (int e = fit_dynamic_smem<paged_attn_kernel<T, D>>(smem, "paged_attention(phase 1)")) return e;
     dim3 grid(p.num_splits, p.nkv, num_seqs);
     paged_attn_kernel<T, D><<<grid, PA_THREADS, smem, stream>>>(p);
     int e = check_launch("paged_attention(phase 1)");

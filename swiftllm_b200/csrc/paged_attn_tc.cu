@@ -448,9 +448,8 @@ bool tc_paged_supported(int head_dim, int block_size, int nq, int nkv, int64_t n
 #define SLLM_TC_LAUNCH(KERNEL, VERIFY, TT, NP)                                                                           \
     do {                                                                                                                 \
         constexpr int smem_bytes = Shape<VERIFY, NP>::SMEM_BYTES;                                                        \
-        static unsigned long long configured = 0;                                                                        \
-        if (first_use_on_this_device(configured))                                                                        \
-            cudaFuncSetAttribute(KERNEL<TT, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);               \
+        const char* what = VERIFY ? "paged_attention_verify(wgmma)" : "paged_attention(wgmma)";                         \
+        if (int e = fit_dynamic_smem<KERNEL<TT, NP>>(smem_bytes, what)) return e;                                        \
         KERNEL<TT, NP><<<grid, TC_THREADS, smem_bytes, a.stream>>>(kmap, vmap, qmap, p);                                 \
     } while (0)
 

@@ -55,9 +55,7 @@ static int launch_gen2(const PrefillLaunch& a) {
     const PfPagedKV& pk = a.paged;
     const PtPaged pg = PAGED ? PtPaged{pk.block_table, pk.seq_ids, pk.prefix_lens, pk.cur_layer, pk.num_layers, pk.max_blocks_per_seq}
                              : PtPaged{};
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(prefill_attn_tc_kernel<T, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM_BYTES);
+    if (int e = fit_dynamic_smem<prefill_attn_tc_kernel<T, PAGED>>(PT_SMEM_BYTES, entry_name<PAGED>)) return e;
     dim3 grid(cdiv(a.max_len, PT_BQ), a.nq, a.num_seqs);
     prefill_attn_tc_kernel<T, PAGED><<<grid, PT_THREADS, PT_SMEM_BYTES, a.stream>>>(qmap, kmap, vmap, p, pg);
     return check_launch(PAGED ? "prefill_attention_paged(wgmma)" : "prefill_attention(wgmma)");
@@ -66,9 +64,7 @@ static int launch_gen2(const PrefillLaunch& a) {
 template <typename T, int D, bool PAGED>
 static int launch_gen1(const PrefillLaunch& a) {
     const size_t smem = (size_t)PF_BQ * D * 2 + 2 * 2 * (size_t)PF_BK * D * 2;
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(prefill_attn_kernel<T, D, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (int e = fit_dynamic_smem<prefill_attn_kernel<T, D, PAGED>>(smem, entry_name<PAGED>)) return e;
     dim3 grid(cdiv(a.max_len, PF_BQ), a.nq, a.num_seqs);
     prefill_attn_kernel<T, D, PAGED><<<grid, PF_THREADS, smem, a.stream>>>((const T*)a.q, (const T*)a.k, (const T*)a.v, (T*)a.o,
                                                                            a.start_locs, a.seq_lens, a.scale_log2e, a.nq, a.nkv,

@@ -162,10 +162,8 @@ __global__ void __launch_bounds__(kRowThreads, 2) prompt_logprobs_kernel(
 template <typename T>
 int launch(const void* logits, int64_t rows, int V, int64_t row_stride, const int32_t* target_ids, int top_n, float* out_logprob,
            int32_t* out_rank, int32_t* out_top_ids, float* out_top_logprobs, cudaStream_t stream) {
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(prompt_logprobs_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageKeys * 2);
     const int stage_vecs = min(kStageKeys, V) / 8;
+    if (int e = fit_dynamic_smem<prompt_logprobs_kernel<T>>((size_t)stage_vecs * 16, "prompt_logprobs")) return e;
     prompt_logprobs_kernel<T><<<(unsigned)rows, kRowThreads, (size_t)stage_vecs * 16, stream>>>(
         (const T*)logits, row_stride, V, stage_vecs, target_ids, top_n, out_logprob, out_rank, out_top_ids, out_top_logprobs);
     return check_launch("prompt_logprobs");

@@ -3,8 +3,8 @@
 // path here) run back to back on the same [Bd, (nq + 2 nkv) * D] rows, 2 x 32 launches per decode step.
 // One thread per (token, head, 8-wide chunk of the first half of the head):
 //   q heads: rotated in place;   k heads: rotated, written in place AND to their cache slot;   v heads: copied to the cache.
-// Same arithmetic as rotary_kernel (elementwise.cu): every product and sum individually rounded (bit-exact with the
-// reference's interpreter and the oracle).  Bytes: 2*T*(nq+nkv)*D*s (rotary) + 4*T*nkv*D*s (store) + T*D*s (cos/sin).
+// Same arithmetic as rotary_kernel (elementwise.cu), rotate8 (common.cuh): every product and sum individually rounded
+// (bit-exact with the reference's interpreter and the oracle).  Bytes: 2*T*(nq+nkv)*D*s (rotary) + 4*T*nkv*D*s (store) + T*D*s (cos/sin).
 #include "common.cuh"
 
 namespace sllm {
@@ -28,11 +28,7 @@ __global__ void __launch_bounds__(256) rotary_store_decode_kernel(
         Vec8<T> x0 = ld_vec8(base + 8 * c), x1 = ld_vec8(base + half + 8 * c);
         Vec8<T> cv = ld_vec8(cosb + t * half + 8 * c), sv = ld_vec8(sinb + t * half + 8 * c);
         Vec8<T> o0, o1;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            o0.v[j] = __hsub2_rn(__hmul2_rn(x0.v[j], cv.v[j]), __hmul2_rn(x1.v[j], sv.v[j]));
-            o1.v[j] = __hadd2_rn(__hmul2_rn(x0.v[j], sv.v[j]), __hmul2_rn(x1.v[j], cv.v[j]));
-        }
+        rotate8(o0, o1, x0, x1, cv, sv);
         st_vec8(base + 8 * c, o0);
         st_vec8(base + half + 8 * c, o1);
         return;
@@ -48,11 +44,7 @@ __global__ void __launch_bounds__(256) rotary_store_decode_kernel(
         Vec8<T> x0 = ld_vec8(base + 8 * c), x1 = ld_vec8(base + half + 8 * c);
         Vec8<T> cv = ld_vec8(cosb + t * half + 8 * c), sv = ld_vec8(sinb + t * half + 8 * c);
         Vec8<T> o0, o1;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            o0.v[j] = __hsub2_rn(__hmul2_rn(x0.v[j], cv.v[j]), __hmul2_rn(x1.v[j], sv.v[j]));
-            o1.v[j] = __hadd2_rn(__hmul2_rn(x0.v[j], sv.v[j]), __hmul2_rn(x1.v[j], cv.v[j]));
-        }
+        rotate8(o0, o1, x0, x1, cv, sv);
         st_vec8(base + 8 * c, o0);
         st_vec8(base + half + 8 * c, o1);
         st_vec8(k_cache + dst + 8 * c, o0);

@@ -257,13 +257,10 @@ inline ClusterGeometry cluster_geometry(int64_t rows, int V, int bytes_per_entry
     return {c, (int)slice_of(V, c, align)};
 }
 
-// Launches Kernel on rows * C CTAs of kThreads in clusters of C, with smem_bytes of dynamic shared memory.  Kernel is a
-// template argument so that each kernel has its own once-per-device flag for the shared-memory attribute.
+// Launches Kernel on rows * C CTAs of kThreads in clusters of C, with smem_bytes of dynamic shared memory
 template <auto Kernel, typename... Args>
 int launch_cluster(int64_t rows, int C, size_t smem_bytes, cudaStream_t stream, const char* name, Args... args) {
-    static unsigned long long configured = 0;
-    if (first_use_on_this_device(configured))
-        cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSliceBytes);
+    if (int e = fit_dynamic_smem<Kernel>(smem_bytes, name)) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(rows * C));
     cfg.blockDim = dim3(kThreads);

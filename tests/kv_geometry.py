@@ -3,9 +3,10 @@ csrc/rotary_store.cu) and of the launchers that size dynamic shared memory near 
 tests can pick shapes that run each regime and name their cases by it.  tests/test_kv_geometry_cpu.py holds this file to the
 sources.
 
+Every launcher with dynamic shared memory raises its kernel's limit through fit_dynamic_smem (csrc/common.cuh) once dynamic
+plus static shared memory pass the 48 KB default; the static size is the compiled kernel's, which STATIC_SMEM states.
 allocate_blocks_kernel (one CTA of ALLOC_THREADS threads) keeps start[batch + 1] and have[batch] in (2 * batch + 1) int32 of
-dynamic shared memory.  Its launcher refuses more than ALLOC_SMEM_MAX bytes and raises the kernel's limit once dynamic plus
-static shared memory pass the 48 KB default.  Step 1 scans the batch ALLOC_THREADS entries at a time; steps 2 and 3 walk the
+dynamic shared memory.  Its launcher refuses more than ALLOC_SMEM_MAX bytes.  Step 1 scans the batch ALLOC_THREADS entries at a time; steps 2 and 3 walk the
 free map ALLOC_WINDOW blocks at a time (16 per thread).
 copy_block_tails_kernel moves one TAIL_CHUNK of a page per CTA.  swap_blocks_gather_kernel cuts each page into SW_SPLIT slices
 of ceil(vecs / SW_SPLIT) 16-byte vectors; a thread moves vectors i and i + SW_THREADS of its slice per iteration."""
@@ -13,21 +14,14 @@ from __future__ import annotations
 
 SMEM_DEFAULT = 48 * 1024              # shared memory (static + dynamic) a kernel may use without cudaFuncSetAttribute
 # static shared memory of each kernel launched with dynamic shared memory that can cross 48 KB, as ptxas lays it out
+# (rmsnorm_kernel<QUANT>: its quantizing instances)
 STATIC_SMEM = {"allocate_blocks_kernel": 144,               # warp_sums[32], s_err
                "allreduce_add_rmsnorm_kernel": 64,          # red[16]
                "allreduce_add_rmsnorm_2shot_kernel": 80,    # red[16], s_last
                "allreduce_add_rmsnorm_ll_kernel": 64,       # red[16]
                "rmsnorm_kernel": 64,                        # red[16]
-               "add_rmsnorm_quant_kernel": 128,             # red[16], redmax[16]
+               "rmsnorm_kernel<QUANT>": 128,                # red[16], redmax[16]
                "silu_and_mul_quant_kernel": 64}             # redmax[16]
-# static shared memory each launcher adds to the dynamic part in its 48 KB test (launch_exchange serves three kernels)
-COUNTED_STATIC = {"allocate_blocks_kernel": 144,
-                  "allreduce_add_rmsnorm_kernel": 80,
-                  "allreduce_add_rmsnorm_2shot_kernel": 80,
-                  "allreduce_add_rmsnorm_ll_kernel": 80,
-                  "rmsnorm_kernel": 64,
-                  "add_rmsnorm_quant_kernel": 128,
-                  "silu_and_mul_quant_kernel": 64}
 
 ALLOC_THREADS = 1024
 ALLOC_WINDOW = ALLOC_THREADS * 16
@@ -51,20 +45,19 @@ def alloc_smem(batch: int) -> int:
     return (2 * batch + 1) * 4
 
 
+def alloc_needs_raise(batch: int) -> bool:
+    """Whether the launch fails unless the limit is raised."""
+    return alloc_smem(batch) + STATIC_SMEM["allocate_blocks_kernel"] > SMEM_DEFAULT
+
+
 def alloc_band(batch: int) -> str:
     """'default' (fits the 48 KB default), 'raised' (the launcher raises the limit) or 'refused' (the launcher refuses)."""
-    smem = alloc_smem(batch)
-    if smem > ALLOC_SMEM_MAX:
+    if alloc_smem(batch) > ALLOC_SMEM_MAX:
         return "refused"
-    return "raised" if smem + COUNTED_STATIC["allocate_blocks_kernel"] > SMEM_DEFAULT else "default"
+    return "raised" if alloc_needs_raise(batch) else "default"
 
 
 MAX_ALLOC_BATCH = max(b for b in range(1, 1 << 16) if alloc_band(b) != "refused")
-
-
-def alloc_needs_raise(batch: int) -> bool:
-    """Whether the launch fails unless the limit is raised: what the hardware counts, not what the launcher counts."""
-    return alloc_smem(batch) + STATIC_SMEM["allocate_blocks_kernel"] > SMEM_DEFAULT
 
 
 def scan_passes(batch: int) -> int:
@@ -111,10 +104,6 @@ def rotary_store_grid(num_seqs: int, nq: int, nkv: int, D: int) -> int:
 # ----------------------------------------------------------------------------- exchange
 def exchange_needs_raise(H: int, kernel: str) -> bool:
     return (H // 8) * 16 + STATIC_SMEM[kernel] > SMEM_DEFAULT
-
-
-def exchange_raises(H: int, kernel: str) -> bool:
-    return (H // 8) * 16 + COUNTED_STATIC[kernel] > SMEM_DEFAULT
 
 
 LL_MAX_HIDDEN = SMEM_DEFAULT // 16 * 8          # the LL launcher refuses a row of more than 48 KB

@@ -1,19 +1,19 @@
-"""TEST INFRASTRUCTURE: the host-side launch geometry of the row kernels (csrc/elementwise.cu: launch_rmsnorm; csrc/fp8.cu:
-launch_add_rmsnorm_quant; csrc/common.cuh: row_threads), restated so that tests can pick widths that run each instance and name
-their cases by it.  tests/test_row_geometry_cpu.py holds this file to the sources.
+"""TEST INFRASTRUCTURE: the host-side launch geometry of the row kernels (csrc/elementwise.cu: launch_rmsnorm, which serves
+RMSNorm, add + RMSNorm and its FP8 variant; csrc/common.cuh: row_threads), restated so that tests can pick widths that run each
+instance and name their cases by it.  tests/test_row_geometry_cpu.py holds this file to the sources.
 
-Both launchers choose one of three instances of their kernel from the row width H alone (nvec = H / 8 16-byte vectors):
+The launcher chooses one of three instances of rmsnorm_kernel from the row width H alone (nvec = H / 8 16-byte vectors):
     VPT = 4   nvec / 4 threads, each keeps 4 vectors in registers     H % 1024 == 0, 2048 <= H <= 8192
     VPT = 2   nvec / 2 threads, each keeps 2 vectors in registers     H % 512 == 0, H <= 4096, not the above
-    VPT = 0   row_threads(nvec) threads, the row staged in nvec * 16 bytes of dynamic shared memory; above 48 KB the launcher
-              raises the kernel's dynamic shared-memory limit first (cudaFuncSetAttribute).  The 48 KB include the kernel's
-              static shared memory, which differs between the two kernels (STATIC_SMEM): at H = 24576 (exactly 48 KB of row)
-              both raise it, at H = 24544 only the FP8 kernel does."""
+    VPT = 0   row_threads(nvec) threads, the row staged in nvec * 16 bytes of dynamic shared memory; once that and the kernel's
+              static shared memory pass 48 KB, the launch raises the kernel's dynamic shared-memory limit first.  The static size
+              differs between the 16-bit and the FP8 instances (STATIC_SMEM): at H = 24576 (exactly 48 KB of row) both raise it,
+              at H = 24544 only the FP8 instance does."""
 from __future__ import annotations
 
 SMEM_DEFAULT = 48 * 1024              # shared memory (static + dynamic) a kernel may use without cudaFuncSetAttribute
 STATIC_SMEM = {"rmsnorm": 16 * 4,     # rmsnorm_kernel: red[16]
-               "add_rmsnorm_quant": 32 * 4}   # add_rmsnorm_quant_kernel: red[16], redmax[16]
+               "rmsnorm_quant": 32 * 4}       # its FP8 instances: red[16], redmax[16]
 VEC = 8                               # 16-bit elements per 16-byte vector
 
 

@@ -1,7 +1,6 @@
-"""CPU: tests/kv_geometry.py against the sources it restates (csrc/kvcache.cu, csrc/swap_gather.cu, csrc/rotary_store.cu, and
-the 48 KB tests of csrc/exchange.cuh, csrc/allreduce_ll.cu, csrc/elementwise.cu and csrc/fp8.cu), the static shared memory
-those launchers count against what ptxas reports for their kernels, and the case tables tests/test_kv_block_kernels_gpu.py
-runs."""
+"""CPU: tests/kv_geometry.py against the sources it restates (csrc/kvcache.cu, csrc/swap_gather.cu, csrc/rotary_store.cu,
+csrc/allreduce_ll.cu's own row limit, and the one rule every launcher follows for the 48 KB shared-memory default), its static
+shared memory against what ptxas reports for the kernels, and the case tables tests/test_kv_block_kernels_gpu.py runs."""
 import os
 import re
 import shutil
@@ -19,7 +18,8 @@ CUOBJDUMP = os.path.join(os.path.dirname(NVCC), "cuobjdump")
 # the source of each kernel whose launcher can cross 48 KB of dynamic shared memory
 KERNEL_SOURCES = {"allocate_blocks_kernel": "kvcache.cu", "allreduce_add_rmsnorm_kernel": "allreduce_norm.cu",
                   "allreduce_add_rmsnorm_2shot_kernel": "allreduce_norm.cu", "allreduce_add_rmsnorm_ll_kernel": "allreduce_ll.cu",
-                  "rmsnorm_kernel": "elementwise.cu", "add_rmsnorm_quant_kernel": "fp8.cu", "silu_and_mul_quant_kernel": "fp8.cu"}
+                  "rmsnorm_kernel": "elementwise.cu", "rmsnorm_kernel<QUANT>": "elementwise.cu",
+                  "silu_and_mul_quant_kernel": "fp8.cu"}
 
 
 def _one(pattern: str, text: str, what: str):
@@ -28,35 +28,31 @@ def _one(pattern: str, text: str, what: str):
     return found[0]
 
 
-def _floats(expr: str) -> int:
-    """Bytes of an `N * sizeof(float)` term."""
-    return int(expr) * 4
-
-
-def counted_static(csrc: str) -> dict:
-    """Static shared memory each launcher adds to its dynamic shared memory in its 48 KB test, read from the sources."""
-    read = lambda f: open(os.path.join(csrc, f)).read()
-    kv, ex, ew, f8 = read("kvcache.cu"), read("exchange.cuh"), read("elementwise.cu"), read("fp8.cu")
-    alloc = int(_one(r"if \(smem \+ (\d+) > 48 \* 1024\)\s*cudaFuncSetAttribute\(allocate_blocks_kernel,", kv, "allocator"))
-    exch = int(_one(r"if \(smem \+ (\d+) > 48 \* 1024\) cudaFuncSetAttribute\(k,", ex, "launch_exchange"))
-    rms = _floats(_one(r"if \(smem \+ (\d+) \* sizeof\(float\) > 48 \* 1024\)\s*cudaFuncSetAttribute\(rmsnorm_kernel<", ew, "rmsnorm"))
-    arq = _floats(_one(r"if \(smem \+ (\d+) \* sizeof\(float\) > 48 \* 1024\)\s*cudaFuncSetAttribute\(add_rmsnorm_quant_kernel<",
-                       f8, "add_rmsnorm_quant"))
-    smq = _floats(_one(r"if \(smem \+ (\d+) \* sizeof\(float\) > 48 \* 1024\)[^\n]*\n\s*cudaFuncSetAttribute\(silu_and_mul_quant_kernel<",
-                       f8, "silu_and_mul_quant"))
-    return {"allocate_blocks_kernel": alloc, "allreduce_add_rmsnorm_kernel": exch, "allreduce_add_rmsnorm_2shot_kernel": exch,
-            "allreduce_add_rmsnorm_ll_kernel": exch, "rmsnorm_kernel": rms, "add_rmsnorm_quant_kernel": arq,
-            "silu_and_mul_quant_kernel": smq}
+def limit_rule_breaches(csrc: str) -> list:
+    """The one shared-memory limit rule: the attribute is set only by raise_dynamic_smem (host.cu), which takes the kernel's
+    static size from the compiled kernel; no launcher sets it, counts static shared memory or keeps a flag of its own."""
+    texts = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh"))}
+    bad = []
+    sets = {f: t.count("cudaFuncAttributeMaxDynamicSharedMemorySize") for f, t in texts.items()}
+    if {f: n for f, n in sets.items() if n} != {"host.cu": 1}:
+        bad.append(("the attribute is set outside raise_dynamic_smem", sets))
+    if any("first_use_on_this_device" in t for t in texts.values()):
+        bad.append("first_use_on_this_device")
+    if re.findall(r"\bsmem\b[^;\n]*[<>]=? 48 \* 1024", "".join(texts.values())):
+        bad.append("a launcher's own 48 KB test")
+    try:
+        _one(r"e = cudaFuncGetAttributes\(&fa, kernel\);\s*limit = 48 \* 1024 - \(int\)fa\.sharedSizeBytes;", texts["host.cu"],
+             "static size of the compiled kernel")
+    except AssertionError as e:
+        bad.append(str(e))
+    return bad
 
 
 def mismatches(csrc: str) -> list:
     read = lambda f: open(os.path.join(csrc, f)).read()
     kv, sw, rs, ll = read("kvcache.cu"), read("swap_gather.cu"), read("rotary_store.cu"), read("allreduce_ll.cu")
-    bad = []
+    bad = limit_rule_breaches(csrc)
     try:
-        got = counted_static(csrc)
-        if got != KG.COUNTED_STATIC:
-            bad.append(("counted static shared memory", got))
         # allocator: shared-memory size, refusal, block shape, windows
         _one(r"const size_t smem = \(size_t\)\(2 \* batch \+ 1\) \* sizeof\(int32_t\);", kv, "allocator smem")
         if int(_one(r"SLLM_REQUIRE\(smem <= (\d+) \* 1024, \"allocate_blocks: batch", kv, "allocator cap")) * 1024 != KG.ALLOC_SMEM_MAX:
@@ -110,10 +106,17 @@ def test_the_mirror_states_the_sources():
 
 
 @pytest.mark.parametrize("edit", [
-    ("kvcache.cu", "if (smem + 144 > 48 * 1024)", "if (smem > 48 * 1024)"),
-    ("exchange.cuh", "if (smem + 80 > 48 * 1024)", "if (smem + 64 > 48 * 1024)"),
-    ("elementwise.cu", "if (smem + 16 * sizeof(float) > 48 * 1024)", "if (smem > 48 * 1024)"),
-    ("fp8.cu", "if (smem + 32 * sizeof(float) > 48 * 1024)", "if (smem + 16 * sizeof(float) > 48 * 1024)"),
+    ("kvcache.cu", "    if (int e = fit_dynamic_smem<allocate_blocks_kernel>(smem, \"allocate_blocks_for_seqs\")) return e;\n",
+     "    if (smem + 144 > 48 * 1024) cudaFuncSetAttribute(allocate_blocks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);\n"),
+    ("exchange.cuh", "if (int e = dtype == SLLM_F16 ? fit_dynamic_smem<F16>(smem, kernel) : fit_dynamic_smem<BF16>(smem, kernel)) return e;",
+     "if (smem + 80 > 48 * 1024) cudaFuncSetAttribute(F16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);"),
+    ("elementwise.cu", "if (int e = fit_dynamic_smem<rmsnorm_kernel<T, FUSED, 0, QUANT>>(smem, what)) return e;",
+     "if (smem + 64 > 48 * 1024) return 1;"),
+    ("fp8.cu", "if (int e = fit_dynamic_smem<silu_and_mul_quant_kernel<T>>(smem, \"silu_and_mul_quant_fp8\")) return e;",
+     "if (smem + 16 * sizeof(float) > 48 * 1024) return 1;"),
+    ("prompt_logprobs.cu", "    const int stage_vecs", "    static unsigned long long configured = 0;\n"
+     "    if (first_use_on_this_device(configured)) {}\n    const int stage_vecs"),
+    ("host.cu", "limit = 48 * 1024 - (int)fa.sharedSizeBytes;", "limit = 48 * 1024 - 64;"),
     ("kvcache.cu", "smem <= 200 * 1024", "smem <= 220 * 1024"),
     ("kvcache.cu", "(int64_t)blockDim.x * 16;", "(int64_t)blockDim.x * 32;"),
     ("kvcache.cu", "if (tgt > mbps) atomicOr(&s_err, 4);", "if (tgt >= mbps) atomicOr(&s_err, 4);"),
@@ -122,8 +125,8 @@ def test_the_mirror_states_the_sources():
     ("swap_gather.cu", "const int64_t j = i + SW_THREADS;", "const int64_t j = i + 2 * SW_THREADS;"),
     ("rotary_store.cu", "const int threads = 256;", "const int threads = 128;"),
     ("allreduce_ll.cu", "sizeof(uint4) <= 48 * 1024", "sizeof(uint4) <= 56 * 1024")],
-    ids=["alloc-48K", "exchange-48K", "rmsnorm-48K", "fp8-48K", "alloc-cap", "alloc-window", "alloc-flag4", "tail-unroll",
-         "swap-split", "swap-second", "rotary-threads", "ll-limit"])
+    ids=["alloc-own-limit", "exchange-own-limit", "rmsnorm-own-limit", "fp8-own-limit", "first-use", "hand-counted-static",
+         "alloc-cap", "alloc-window", "alloc-flag4", "tail-unroll", "swap-split", "swap-second", "rotary-threads", "ll-limit"])
 def test_a_changed_source_is_noticed(tmp_path, edit):
     f, old, new = edit
     for name in os.listdir(CSRC):
@@ -133,6 +136,14 @@ def test_a_changed_source_is_noticed(tmp_path, edit):
     assert text.count(old) == 1
     (tmp_path / f).write_text(text.replace(old, new))
     assert mismatches(str(tmp_path)) != []
+
+
+def _mangled(kernel: str) -> str:
+    """Pattern of the mangled names of a KERNEL_SOURCES entry's instances: rmsnorm_kernel's last template argument (QUANT)
+    tells its quantizing instances from the others."""
+    if kernel.startswith("rmsnorm_kernel"):
+        return r"\drmsnorm_kernelI\w*?Lb%dEEEv" % kernel.endswith("<QUANT>")
+    return r"\d" + kernel
 
 
 def static_smem_of_cubins(csrc: str, out_dir) -> dict:
@@ -150,20 +161,18 @@ def static_smem_of_cubins(csrc: str, out_dir) -> dict:
         dumps = dict(zip(files, ex.map(compile_one, files)))
     sizes = {}
     for kernel, f in KERNEL_SOURCES.items():
-        found = re.findall(r"Function (\S*?\d" + kernel + r"\S*):\s*\n\s*REG:\d+ STACK:\d+ SHARED:(\d+) ", dumps[f])
+        found = re.findall(r"Function (\S*?" + _mangled(kernel) + r"\S*):\s*\n\s*REG:\d+ STACK:\d+ SHARED:(\d+) ", dumps[f])
         assert found, f"{kernel} not in the cubin of {f}"
         sizes[kernel] = {int(s) - 1024 for _, s in found}
     return sizes
 
 
 @pytest.mark.skipif(not (os.path.exists(NVCC) and os.path.exists(CUOBJDUMP)), reason="needs nvcc and cuobjdump")
-def test_launchers_count_at_least_the_static_shared_memory_ptxas_reports(tmp_path):
-    """What keeps the bug class away: each launcher that can pass 48 KB of dynamic shared memory raises the limit once dynamic
-    plus static shared memory pass 48 KB, so the static size it counts must not be less than what the kernel really has."""
+def test_the_static_shared_memory_is_what_ptxas_reports(tmp_path):
+    """STATIC_SMEM puts the GPU tests' edge cases (the allocator's B6126-edge ... B6143, the exchange widths 24544 ... 24576,
+    the rows of tests/row_geometry.py) exactly where the launchers start to raise the limit."""
     sizes = static_smem_of_cubins(CSRC, tmp_path)
     assert sizes == {k: {v} for k, v in KG.STATIC_SMEM.items()}, sizes
-    counted = counted_static(CSRC)
-    assert all(counted[k] >= KG.STATIC_SMEM[k] for k in KG.STATIC_SMEM), counted
 
 
 def test_the_allocator_bands():
@@ -180,8 +189,6 @@ def test_the_exchange_bands():
     band = lambda k: [H for H in range(8, 65537, 8) if KG.exchange_needs_raise(H, k) and (H // 8) * 16 <= KG.SMEM_DEFAULT]
     assert band("allreduce_add_rmsnorm_kernel") == band("allreduce_add_rmsnorm_ll_kernel") == list(range(24552, 24577, 8))
     assert band("allreduce_add_rmsnorm_2shot_kernel") == list(range(24544, 24577, 8))
-    assert all(KG.exchange_raises(H, k) for k in KG.STATIC_SMEM if k.startswith("allreduce") for H in range(8, 65537, 8)
-               if KG.exchange_needs_raise(H, k))
     assert KG.LL_MAX_HIDDEN == 24576
 
 

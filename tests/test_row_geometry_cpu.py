@@ -1,5 +1,5 @@
-"""CPU: tests/row_geometry.py against the launchers it restates (csrc/elementwise.cu: launch_rmsnorm, csrc/fp8.cu:
-launch_add_rmsnorm_quant, csrc/common.cuh: row_threads), the width table tests/test_row_kernels_gpu.py runs, and the fp64 bounds
+"""CPU: tests/row_geometry.py against the launcher it restates (csrc/elementwise.cu: launch_rmsnorm, csrc/common.cuh:
+row_threads), the width table tests/test_row_kernels_gpu.py runs, and the fp64 bounds
 of tests/row_oracle.py: they accept the kernels' fp32 arithmetic in their own order and in numpy's, and the GPU tests' data
 rejects plausible wrong variants of it."""
 import os
@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+import kv_geometry as KG
 import row_geometry as RG
 import row_oracle as RO
 
@@ -25,28 +26,24 @@ def _one(pattern: str, text: str, what: str):
     return found[0]
 
 
-def launcher_rules(src: str, kernel: str, threads: str, static_floats: int) -> list:
-    """[(condition, vpt, threads expression)] of a launcher's register instances, in order, after checking that its generic
-    instance stages nvec vectors and raises the shared-memory limit above 48 KB, counting the kernel's static floats."""
-    rules = re.findall(r"if \((nvec [^{]*?)\) \{\s*" + kernel + r"<T, (?:FUSED, )?(\d)><<<\(unsigned\)T_, (nvec / \d), 0, stream>>>",
+def launcher_rules(src: str) -> list:
+    """[(condition, vpt, threads expression)] of launch_rmsnorm's register instances, in order, after checking that its generic
+    instance stages nvec vectors on row_threads(nvec) threads and fits its shared-memory limit to them first."""
+    rules = re.findall(r"if \((nvec [^{]*?)\) \{\s*rmsnorm_kernel<T, FUSED, (\d), QUANT><<<\(unsigned\)T_, (nvec / \d), 0, stream>>>",
                        src)
-    _one(r"smem = \(size_t\)nvec \* sizeof\(uint4\);\s*(?://[^\n]*\s*)?if \(smem \+ " + str(static_floats) +
-         r" \* sizeof\(float\) > 48 \* 1024\)\s*cudaFuncSetAttribute\(" + kernel +
-         r"<T, (?:FUSED, )?0>, cudaFuncAttributeMaxDynamicSharedMemorySize, \(int\)smem\);", src, kernel + " generic smem")
-    _one(kernel + r"<T, (?:FUSED, )?0><<<\(unsigned\)T_, (" + re.escape(threads) + r"), smem, stream>>>", src, kernel + " generic")
+    _one(r"const int threads = row_threads\(nvec\);\s*const size_t smem = \(size_t\)nvec \* sizeof\(uint4\);\s*"
+         r"if \(int e = fit_dynamic_smem<rmsnorm_kernel<T, FUSED, 0, QUANT>>\(smem, what\)\) return e;\s*"
+         r"rmsnorm_kernel<T, FUSED, 0, QUANT><<<\(unsigned\)T_, threads, smem, stream>>>", src, "launch_rmsnorm generic")
     return rules
 
 
 def mismatches(csrc: str) -> list:
     read = lambda f: open(os.path.join(csrc, f)).read()
-    ew = read("elementwise.cu")
     try:
-        _one(r"const int threads = row_threads\(nvec\);", ew, "launch_rmsnorm threads")
-        a = launcher_rules(ew, "rmsnorm_kernel", "threads", RG.STATIC_SMEM["rmsnorm"] // 4)
-        b = launcher_rules(read("fp8.cu"), "add_rmsnorm_quant_kernel", "row_threads(nvec)", RG.STATIC_SMEM["add_rmsnorm_quant"] // 4)
+        a = launcher_rules(read("elementwise.cu"))
     except AssertionError as e:          # a launch statement the patterns no longer find
         return [str(e)]
-    bad = [] if a == b else [("the launchers differ", a, b)]
+    bad = []
     if [(v, t) for _, v, t in a] != [("4", "nvec / 4"), ("2", "nvec / 2")]:
         bad.append(("instances", a))
     # the sources' own conditions pick the instance the mirror picks, at every width the C ABI takes
@@ -64,15 +61,19 @@ def mismatches(csrc: str) -> list:
 
 def test_the_mirror_states_the_launchers():
     assert mismatches(CSRC) == []
+    assert RG.STATIC_SMEM == {"rmsnorm": KG.STATIC_SMEM["rmsnorm_kernel"], "rmsnorm_quant": KG.STATIC_SMEM["rmsnorm_kernel<QUANT>"]}
 
 
 @pytest.mark.parametrize("edit", [("elementwise.cu", "(nvec / 2) % 32 == 0 && nvec / 2 <= 256", "(nvec / 2) % 32 == 0 && nvec / 2 <= 128"),
-                                  ("fp8.cu", "nvec / 4 >= 64 && nvec / 4 <= 256", "nvec / 4 >= 32 && nvec / 4 <= 256"),
-                                  ("fp8.cu", "if (smem + 32 * sizeof(float) > 48 * 1024)", "if (smem > 48 * 1024)"),
-                                  ("elementwise.cu", "if (smem + 16 * sizeof(float) > 48 * 1024)", "if (smem > 48 * 1024)"),
-                                  ("fp8.cu", "T_, row_threads(nvec), smem", "T_, row_threads(nvec / 2), smem"),
+                                  ("elementwise.cu", "nvec / 4 >= 64 && nvec / 4 <= 256", "nvec / 4 >= 32 && nvec / 4 <= 256"),
+                                  ("elementwise.cu", "const int threads = row_threads(nvec);", "const int threads = row_threads(nvec / 2);"),
+                                  ("elementwise.cu", "const size_t smem = (size_t)nvec * sizeof(uint4);",
+                                   "const size_t smem = (size_t)nvec * 8;"),
+                                  ("elementwise.cu", "    if (int e = fit_dynamic_smem<rmsnorm_kernel<T, FUSED, 0, QUANT>>(smem, what)) return e;\n", ""),
+                                  ("elementwise.cu", "rmsnorm_kernel<T, FUSED, 4, QUANT><<<(unsigned)T_, nvec / 4,",
+                                   "rmsnorm_kernel<T, FUSED, 4, QUANT><<<(unsigned)T_, nvec / 2,"),
                                   ("common.cuh", "nvec >= 256 ? 256", "nvec >= 128 ? 128")],
-                         ids=["vpt2-range", "fp8-vpt4-range", "fp8-smem", "smem", "fp8-threads", "row_threads"])
+                         ids=["vpt2-range", "vpt4-range", "threads", "generic-smem", "generic-limit", "vpt4-threads", "row_threads"])
 def test_a_changed_launcher_is_noticed(tmp_path, edit):
     f, old, new = edit
     for name in os.listdir(CSRC):
@@ -98,8 +99,8 @@ def test_the_width_table_covers_every_instance():
     assert RG.launch_path(1040) == (0, 160, 130 * 16, False) and 1040 in by["GEN"]
     assert RG.launch_path(8200) == (0, 512, 1025 * 16, False) and 8200 in by["GEN"]
     assert RG.launch_path(24544) == (0, 512, 48 * 1024 - 64, False) and 24544 in by["GEN"]
-    assert RG.launch_path(24552)[3] and RG.launch_path(24528, "add_rmsnorm_quant")[3]
-    assert not RG.launch_path(24512, "add_rmsnorm_quant")[3]
+    assert RG.launch_path(24552)[3] and RG.launch_path(24528, "rmsnorm_quant")[3]
+    assert not RG.launch_path(24512, "rmsnorm_quant")[3]
     assert RG.launch_path(24576) == (0, 512, 48 * 1024, True) and 24576 in by["GEN>48K"]
     assert RG.launch_path(28672) == (0, 512, 3584 * 16, True) and 28672 in by["GEN>48K"]
     assert RG.launch_path(64) == (0, 32, 128, False)
