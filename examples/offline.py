@@ -11,6 +11,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --logprobs 5       print each generated token's log-probability and the 5 most likely tokens (forward_with_logprobs)
     ... --prompt-logprobs 3    print each prompt's perplexity and the 3 most likely tokens at its first positions
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
+    ... --no-repeat-ngram 3 / --dry-multiplier 0.8 [--dry-breakers 198 25]    ban repeated 3-grams / DRY phrase-repeat penalty
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
     ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
     ... --lora /data/my-adapter    run every prompt under a PEFT LoRA adapter (load_lora, lora_ids_list)
@@ -160,6 +161,12 @@ def main():
     ap.add_argument("--repetition-penalty", type=float, default=1.0, help="divide / multiply the logits of seen tokens (1 = off)")
     ap.add_argument("--frequency-penalty", type=float, default=0.0, help="subtract this times each token's output count (0 = off)")
     ap.add_argument("--presence-penalty", type=float, default=0.0, help="subtract this from every token already output (0 = off)")
+    ap.add_argument("--no-repeat-ngram", type=int, default=0, help="ban every token that would repeat an n-gram of this size (0 = off)")
+    ap.add_argument("--dry-multiplier", type=float, default=0.0, help="DRY penalty multiplier (0 = off)")
+    ap.add_argument("--dry-base", type=float, default=1.75, help="DRY penalty base")
+    ap.add_argument("--dry-allowed-length", type=int, default=2, help="longest repeat DRY leaves alone")
+    ap.add_argument("--dry-breakers", type=int, nargs="*", default=[],
+                    help="DRY sequence-breaker token ids (the last token of encode('a' + s) for s in '\\n', ':', '\"', '*')")
     ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
     ap.add_argument("--n", type=int, default=1, help="samples per prompt: prefill once, fork n - 1 times, distinct seeds (1 = off)")
     ap.add_argument("--lora", type=str, default=None, help="PEFT LoRA adapter directory: every prompt runs under this adapter")
@@ -171,8 +178,8 @@ def main():
     if not 0 <= args.speculate <= 7:
         ap.error("--speculate takes 0..7 drafts")
     if args.speculate and (args.logprobs is not None or args.prompt_logprobs is not None or args.repetition_penalty != 1.0 or args.frequency_penalty != 0.0
-                           or args.presence_penalty != 0.0):
-        ap.error("--speculate does not combine with --logprobs, --prompt-logprobs or penalties")
+                           or args.presence_penalty != 0.0 or args.no_repeat_ngram or args.dry_multiplier):
+        ap.error("--speculate does not combine with --logprobs, --prompt-logprobs, penalties, --no-repeat-ngram or DRY")
 
     ec = swiftllm_b200.EngineConfig(model_path=args.model_path or "", use_dummy=False, block_size=16, gpu_mem_utilization=0.9,
                                     num_cpu_blocks=0, max_seqs_in_block_table=128, max_blocks_per_seq=2048, max_batch_size=16,
@@ -212,8 +219,12 @@ def main():
     params = swiftllm_b200.SamplingParams(args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed, logprobs=args.logprobs,
                                           prompt_logprobs=args.prompt_logprobs,
                                           repetition_penalty=args.repetition_penalty, frequency_penalty=args.frequency_penalty,
-                                          presence_penalty=args.presence_penalty)
-    if args.temperature == 0 and args.logprobs is None and args.prompt_logprobs is None and not params.has_penalties():
+                                          presence_penalty=args.presence_penalty, no_repeat_ngram_size=args.no_repeat_ngram,
+                                          dry_multiplier=args.dry_multiplier, dry_base=args.dry_base,
+                                          dry_allowed_length=args.dry_allowed_length,
+                                          dry_sequence_breakers=tuple(args.dry_breakers))
+    if (args.temperature == 0 and args.logprobs is None and args.prompt_logprobs is None and not params.has_penalties()
+            and not params.has_ngram_controls()):
         params = None
     logs = [[] for _ in range(len(input_ids) * args.n)]
     prompt_logs = [[] for _ in input_ids]

@@ -331,6 +331,25 @@ int sllm_apply_penalties(void* logits, int64_t num_rows, int vocab_size, int64_t
                          const int32_t* block_table, int block_table_stride, int block_size, int32_t* token_cache,
                          int64_t num_blocks, sllm_dtype_t dtype, sllm_stream_t stream);
 
+/* ---- N-gram repetition controls (new): sllm_apply_penalties plus a no-repeat n-gram ban and the DRY penalty, from the same one
+ * read of the history in the same launch.  Extra per-row DEVICE arrays [num_rows]: no_repeat_ngram_size n (0: no ban),
+ * dry_allowed_length A, dry_multiplier (0: no DRY), dry_base, and dry_breakers int32 [num_rows, 16] (global ids, -1 unused).
+ * With x[0, L) the history (L = pos, ids compared without the output bit; unmapped positions match nothing), m(j) the longest
+ * m <= min(j, 50) with x[j - k] == x[L - k] for k = 1 .. m, and M(v) the largest m(j) over the j with x[j] == v: the ban sets
+ * l = -inf where M(v) >= n - 1; DRY, with b the smallest k >= 1 such that x[L - k] is a breaker (infinite if none) and
+ * D(v) = min(M(v), b - 1) for a v that is no breaker, subtracts q = multiplier * base^(D - A) (fp32, multiplied out in order)
+ * where D >= A.  Per entry: the penalties (rows with any of them), DRY, the ban, one rounding; untouched entries keep their
+ * bits.  A row with all eight controls off is skipped.  8-byte cluster slots: vocab_size up to about 204k entries.  Rejected
+ * before launch: what sllm_apply_penalties rejects, and null control arrays. */
+int sllm_apply_penalties_ngram(void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                               int64_t vocab_offset, const float* repetition_penalty, const float* frequency_penalty,
+                               const float* presence_penalty, const int32_t* seq_ids, const int32_t* pos,
+                               const int32_t* input_ids, const int32_t* last_token_indices, const int32_t* prefill_seq_lens,
+                               int num_prefill_rows, const int32_t* block_table, int block_table_stride, int block_size,
+                               int32_t* token_cache, int64_t num_blocks, const int32_t* no_repeat_ngram_size,
+                               const int32_t* dry_allowed_length, const float* dry_multiplier, const float* dry_base,
+                               const int32_t* dry_breakers, sllm_dtype_t dtype, sllm_stream_t stream);
+
 /* ---- Constrained decoding (new): allowed-token bitmasks and logit bias, IN PLACE on logits laid out as in sllm_sample_tokens
  * (a vocabulary shard with vocab_offset works; bits and bias ids are global indices).  Per-row DEVICE arrays [num_rows]:
  * mask_index (-1: no mask; else a row of masks uint32 [num_masks, mask_words], bit v % 32 of word v / 32 set = id v allowed)

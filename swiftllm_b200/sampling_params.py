@@ -9,6 +9,8 @@ import torch
 MAX_LOGPROBS = 20                   # csrc/logprobs.cu: kMaxTopN
 MAX_LOGIT_BIAS = 1024               # entries of SamplingParams.logit_bias (csrc/constraints.cu reads them per row)
 MAX_BIAS = 100.0                    # |logit_bias value| bound of the OpenAI API
+MAX_NGRAM = 50                      # csrc/penalties.cu: kMaxMatch, the longest match the n-gram controls see
+MAX_DRY_BREAKERS = 16               # csrc/penalties.cu: kMaxBreakers
 
 
 @dataclasses.dataclass
@@ -35,7 +37,22 @@ class SamplingParams:
     logit_bias (csrc/constraints.cu): None or {token id: bias}, at most MAX_LOGIT_BIAS entries, biases finite in [-100, 100], ids
     in [0, vocab_size) (checked by the step).  Applied after the step's allowed-token mask (token_masks_list of LlamaModel.forward)
     and before the penalties: l = round(float(l) + bias), one fp32 add and one rounding to the storage dtype; a masked id stays
-    -inf.  Log-probabilities stay those of the raw logits."""
+    -inf.  Log-probabilities stay those of the raw logits.
+
+    N-gram repetition controls (csrc/penalties.cu, in the penalty kernel's launch), over the same history as the penalties and
+    with the same contract: pass the same parameters from the request's first prefill chunk on.  With x the prompt and output
+    tokens so far, M(v) is the longest run of tokens (at most 50) that ends the sequence and also ends somewhere before an
+    earlier occurrence of v - the repeat that v would extend.
+    no_repeat_ngram_size n (0: off, at most 50) bans (-inf) every token that would complete an n-gram already in the sequence,
+    M(v) >= n - 1: Hugging Face's NoRepeatNGramLogitsProcessor over prompt + output (n = 1 bans every token seen).
+    dry_multiplier (0: off), dry_base, dry_allowed_length A and dry_sequence_breakers are text-generation-webui's DRY ("Don't
+    Repeat Yourself") over the whole history: a token that is no breaker and would extend a repeat of D >= A tokens, where the
+    repeat is cut at the nearest breaker among the last tokens, loses multiplier * base^(D - A) (fp32, multiplied out in order).
+    The breakers are token ids (at most 16, each < vocab_size, checked by the step); text-generation-webui's defaults are, for
+    each string s of ["\n", ":", "\"", "*"], the last token id of tokenizer.encode("a" + s).
+    The order per token is: penalties, DRY, ban, one rounding to the storage dtype; they run after the mask and logit_bias.  A
+    row whose mask and bans leave no token allowed gets the all -inf row rule of the token choice.  Log-probabilities stay those
+    of the raw logits.  forward_speculative and ignore_kvcache raise ValueError for them, as for the penalties."""
     temperature: float = 0.0
     top_k: int = 0
     top_p: float = 1.0
@@ -46,6 +63,11 @@ class SamplingParams:
     frequency_penalty: float = 0.0
     presence_penalty: float = 0.0
     logit_bias: Optional[dict] = None
+    no_repeat_ngram_size: int = 0
+    dry_multiplier: float = 0.0
+    dry_base: float = 1.75
+    dry_allowed_length: int = 2
+    dry_sequence_breakers: tuple = ()
 
     def validate(self):
         if not (isinstance(self.temperature, (int, float)) and math.isfinite(self.temperature) and self.temperature >= 0):
@@ -78,9 +100,31 @@ class SamplingParams:
                     raise ValueError(f"logit_bias keys must be token ids (integers >= 0), got {k!r}")
                 if not (_is_real(v) and math.isfinite(v) and -MAX_BIAS <= v <= MAX_BIAS):
                     raise ValueError(f"logit_bias values must be finite numbers in [-100, 100], got {v!r} for id {k}")
+        for name, lo in (("no_repeat_ngram_size", 0), ("dry_allowed_length", 1)):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= MAX_NGRAM:
+                raise ValueError(f"{name} must be an integer in [{lo}, {MAX_NGRAM}], got {v!r}")
+        if not (_is_real(self.dry_multiplier) and math.isfinite(self.dry_multiplier) and self.dry_multiplier >= 0):
+            raise ValueError(f"dry_multiplier must be a finite number >= 0, got {self.dry_multiplier!r}")
+        if not (_is_real(self.dry_base) and math.isfinite(self.dry_base) and self.dry_base >= 1):
+            raise ValueError(f"dry_base must be a finite number >= 1, got {self.dry_base!r}")
+        br = self.dry_sequence_breakers
+        if not isinstance(br, (tuple, list)):
+            raise ValueError(f"dry_sequence_breakers must be a tuple of token ids, got {type(br).__name__}")
+        if len(br) > MAX_DRY_BREAKERS:
+            raise ValueError(f"dry_sequence_breakers has {len(br)} ids; at most {MAX_DRY_BREAKERS} are supported")
+        for t in br:
+            if isinstance(t, bool) or not isinstance(t, (int, np.integer)) or not 0 <= t < 2 ** 31:
+                raise ValueError(f"dry_sequence_breakers must hold token ids (integers >= 0), got {t!r}")
+        if len(set(int(t) for t in br)) != len(br):
+            raise ValueError(f"dry_sequence_breakers ids must be distinct, got {tuple(br)!r}")
 
     def has_penalties(self) -> bool:
         return self.repetition_penalty != 1.0 or self.frequency_penalty != 0.0 or self.presence_penalty != 0.0
+
+    def has_ngram_controls(self) -> bool:
+        """The no-repeat n-gram ban or DRY is on."""
+        return self.no_repeat_ngram_size > 0 or self.dry_multiplier > 0
 
 
 def _is_real(v) -> bool:
@@ -130,8 +174,10 @@ def _i32(words: np.ndarray) -> list:
 
 def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator):
     """Validates the list and returns the staged int32 words (seed lo/hi interleaved [2B], temperature bits [B], top_k [B],
-    top_p bits [B], and when some row has penalties the fp32 bits of repetition, frequency and presence penalty [3B]) and whether
-    any row filters (top-k / top-p); None when every row is greedy and none has penalties.  Raises ValueError."""
+    top_p bits [B], and when some row has penalties or n-gram controls the fp32 bits of repetition, frequency and presence
+    penalty [3B]; when some row has n-gram controls then no_repeat_ngram_size [B], dry_allowed_length [B], the fp32 bits of
+    dry_multiplier [B] and dry_base [B], and dry_sequence_breakers [B, 16] padded with -1) and whether any row filters (top-k /
+    top-p); None when every row is greedy and none has penalties or n-gram controls.  Raises ValueError."""
     if len(params_list) != batch_size:
         raise ValueError(f"sampling_params_list has {len(params_list)} entries for a batch of {batch_size}")
     for sp in params_list:
@@ -140,7 +186,8 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
         sp.validate()
     # a fresh seed for every unseeded row, drawn even for greedy rows so the stream does not depend on the batch's mix
     seeds = np.array([int(rng.integers(0, 2 ** 63)) if sp.seed is None else int(sp.seed) for sp in params_list], dtype=np.uint64)
-    penalized = any(sp.has_penalties() for sp in params_list)
+    ngram = any(sp.has_ngram_controls() for sp in params_list)
+    penalized = ngram or any(sp.has_penalties() for sp in params_list)
     if not penalized and all(sp.temperature == 0 for sp in params_list):
         return None
     temp = np.array([sp.temperature for sp in params_list], dtype=np.float32)
@@ -151,12 +198,33 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
     if penalized:
         for name in ("repetition_penalty", "frequency_penalty", "presence_penalty"):
             words += _i32(np.array([getattr(sp, name) for sp in params_list], dtype=np.float32).view(np.uint32))
+    if ngram:
+        words += [int(sp.no_repeat_ngram_size) for sp in params_list] + [int(sp.dry_allowed_length) for sp in params_list]
+        for name in ("dry_multiplier", "dry_base"):
+            words += _i32(np.array([getattr(sp, name) for sp in params_list], dtype=np.float32).view(np.uint32))
+        for sp in params_list:
+            br = [int(t) for t in sp.dry_sequence_breakers]
+            words += br + [-1] * (MAX_DRY_BREAKERS - len(br))
     return words, filtered
 
 
 def has_penalties(params_list: Optional[list]) -> bool:
     """Some entry of the (validated) list has a penalty: the step applies them and records its tokens in the token pages."""
     return any(sp.has_penalties() for sp in params_list or [])
+
+
+def has_ngram_controls(params_list: Optional[list]) -> bool:
+    """Some entry of the (validated) list has the n-gram ban or DRY: the penalty kernel's n-gram launch runs, and the step
+    records its tokens in the token pages."""
+    return any(sp.has_ngram_controls() for sp in params_list or [])
+
+
+def check_breaker_ids(params_list: Optional[list], vocab_size: int):
+    """ValueError when a (validated) entry's dry_sequence_breakers holds an id outside [0, vocab_size)."""
+    for i, sp in enumerate(params_list or []):
+        bad = [int(t) for t in sp.dry_sequence_breakers if int(t) >= vocab_size]
+        if bad:
+            raise ValueError(f"sampling_params_list[{i}].dry_sequence_breakers has token id {bad[0]} outside [0, {vocab_size})")
 
 
 def token_mask(vocab_size: int, allowed_ids) -> np.ndarray:

@@ -98,6 +98,12 @@ class SamplingState:
     repetition_penalty: Optional[torch.Tensor] = None   # [batch_size] float32, 1 = off
     frequency_penalty: Optional[torch.Tensor] = None    # [batch_size] float32, 0 = off
     presence_penalty: Optional[torch.Tensor] = None     # [batch_size] float32, 0 = off
+    # ---- n-gram ban and DRY (csrc/penalties.cu); None when no row of the step has them (then the penalties above are staged too)
+    no_repeat_ngram_size: Optional[torch.Tensor] = None     # [batch_size] int32, 0 = off
+    dry_allowed_length: Optional[torch.Tensor] = None       # [batch_size] int32
+    dry_multiplier: Optional[torch.Tensor] = None           # [batch_size] float32, 0 = off
+    dry_base: Optional[torch.Tensor] = None                 # [batch_size] float32
+    dry_breakers: Optional[torch.Tensor] = None             # [batch_size, 16] int32, -1 = unused
     sampled: bool = True            # some row has temperature > 0; False: every row takes the argmax of its penalised logits
     # the token history the penalty kernel reads and extends, set by the model: the step's input ids (int32 [num_tokens]), the
     # block table and the token pages (int32 [num_blocks, block_size])
@@ -109,16 +115,31 @@ class SamplingState:
     def penalized(self) -> bool:
         return self.repetition_penalty is not None
 
+    @property
+    def ngram(self) -> bool:
+        return self.no_repeat_ngram_size is not None
+
+    def ngram_kwargs(self) -> dict:
+        """The n-gram keyword arguments of worker.kernels.penalties.apply_penalties ({} without n-gram controls)."""
+        if not self.ngram:
+            return {}
+        return dict(no_repeat_ngram_size=self.no_repeat_ngram_size, dry_allowed_length=self.dry_allowed_length,
+                    dry_multiplier=self.dry_multiplier, dry_base=self.dry_base, dry_breakers=self.dry_breakers)
+
     @staticmethod
     def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool, sampled: bool = True) -> "SamplingState":
         """`words`: the int32 device view staged from swiftllm_b200.sampling_params.sampling_words (8-byte aligned); 8 * B
-        words carry the penalties after the 5 * B sampling words."""
+        words carry the penalties after the 5 * B sampling words; 28 * B words also the n-gram controls after those."""
         B = pos.shape[0]
         pen = {}
-        if words.shape[0] == 8 * B:
+        if words.shape[0] in (8 * B, 28 * B):
             pen = dict(repetition_penalty=words[5 * B:6 * B].view(torch.float32),
                        frequency_penalty=words[6 * B:7 * B].view(torch.float32),
                        presence_penalty=words[7 * B:8 * B].view(torch.float32))
+        if words.shape[0] == 28 * B:
+            pen.update(no_repeat_ngram_size=words[8 * B:9 * B], dry_allowed_length=words[9 * B:10 * B],
+                       dry_multiplier=words[10 * B:11 * B].view(torch.float32), dry_base=words[11 * B:12 * B].view(torch.float32),
+                       dry_breakers=words[12 * B:28 * B].view(B, 16))
         return SamplingState(temperature=words[2 * B:3 * B].view(torch.float32), top_k=words[3 * B:4 * B],
                              top_p=words[4 * B:5 * B].view(torch.float32), seed=words[:2 * B].view(torch.int64), pos=pos,
                              filtered=filtered, sampled=sampled, **pen)

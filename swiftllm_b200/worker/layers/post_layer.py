@@ -18,7 +18,8 @@ Addition (penalties, csrc/penalties.cu): when some row carries repetition / freq
 the logits the token is chosen from are penalised first (a copy when log-probabilities are asked for: they stay those of the raw
 logits) and the step's tokens are recorded in the token pages.  With a sharded lm_head the pair-merge path penalises each rank's
 shard (vocab_offset) before its local choice; the gather path penalises the gathered full rows on every rank.  Every rank records
-the same tokens in its own pages.
+the same tokens in its own pages.  Rows with the no-repeat n-gram ban or DRY (sampling.ngram) go through the same launch, which
+then also applies those (the kernel's n-gram instantiation); their result does not depend on the shard, so both paths agree.
 
 Addition (prompt log-probabilities, csrc/prompt_logprobs.cu): when the step scores prompt rows (infer_state.prompt_logprobs),
 the last-row path above runs first, unchanged; then the prompt rows go through the final RMSNorm, lm_head (gathered when
@@ -166,7 +167,7 @@ class LlamaPostLayer:
         out = logits.clone() if copy else logits
         apply_penalties(out, sp.repetition_penalty, sp.frequency_penalty, sp.presence_penalty, sp.pos, infer_state.seq_ids,
                         sp.input_ids, last_idx, infer_state.prefill_seq_lens, infer_state.num_prefill_seqs, sp.block_table,
-                        sp.token_cache, vocab_offset=vocab_offset)
+                        sp.token_cache, vocab_offset=vocab_offset, **sp.ngram_kwargs())
         return out
 
     def _gather_logits(self, logits: torch.Tensor) -> torch.Tensor:

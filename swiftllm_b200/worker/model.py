@@ -35,7 +35,8 @@ from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
 from swiftllm_b200.sampling_params import (ConstraintWords, PromptLogprobs, SamplingParams, TokenLogprobs, constraint_words,
-                                           has_penalties, logprobs_top_n, prompt_logprobs_top_n, sampling_words)
+                                           check_breaker_ids, has_ngram_controls, has_penalties, logprobs_top_n,
+                                           prompt_logprobs_top_n, sampling_words)
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker import fp8 as fp8_weights
 from swiftllm_b200.worker.block_manager import BlockManager
@@ -114,7 +115,8 @@ class LlamaModel:
         self.num_blocks = None
         self.k_cache = self.v_cache = None
         self.k_swap = self.v_swap = None
-        # token pages (SamplingParams penalties): written in steps with a penalised row, carried in swaps once one has run
+        # token pages (SamplingParams penalties and n-gram controls): written in steps with such a row, carried in swaps once
+        # one has run
         self.token_cache = self.token_swap = None
         self._penalties_used = False
         self.cpu_block_manager = self.gpu_block_manager = None
@@ -432,8 +434,10 @@ class LlamaModel:
         its temperature / top-k / top-p and seed (csrc/sampling.cu), the noise keyed by the sequence length after this step.
         None (or every temperature 0) is greedy decoding, the reference's behaviour.  Entries with repetition / frequency /
         presence penalties have their logits penalised first (csrc/penalties.cu), over the history recorded in the token pages:
-        such a request must carry the same parameters from its first prefill chunk on.  Invalid parameters (and penalties with
-        ignore_kvcache, which has no block table to record into) raise ValueError before anything is enqueued.
+        such a request must carry the same parameters from its first prefill chunk on.  The no-repeat n-gram ban and DRY
+        (SamplingParams.no_repeat_ngram_size, dry_*) read the same history in the same launch, after the penalties, with the
+        same contract.  Invalid parameters (and penalties or n-gram controls with ignore_kvcache, which has no block table to
+        record into, or a DRY breaker id outside [0, vocab_size)) raise ValueError before anything is enqueued.
 
         `token_masks_list` (addition, constrained decoding): None, or one entry per batch entry - None (unconstrained) or a packed
         allowed-token mask, a numpy array or CPU tensor of int32 / uint32 with W = ceil(vocab_size / 32) words, bit v % 32 of word
@@ -578,7 +582,7 @@ class LlamaModel:
         K/V of rejected rows inside a kept block are overwritten by later steps (attention never reads past a row's position).
         Speculative entries only (no prompts in the same call); runs eagerly and syncs once, like forward().  Raises ValueError
         before anything is enqueued for: a row count outside [1, 8], a negative prefix or one whose rows run past the position
-        table, ignore_kvcache, invalid sampling parameters, and penalties.  SamplingParams.logprobs is ignored.
+        table, ignore_kvcache, invalid sampling parameters, penalties and n-gram controls.  SamplingParams.logprobs is ignored.
 
         token_masks_list: None, or per entry None or a [k + 1, W] mask array (forward()'s layout, one row per input row): row j holds
         the constraint state after x, d_1 .. d_j, the mask the caller would pass to the plain step at that position; the entry's
@@ -601,6 +605,8 @@ class LlamaModel:
         samp = None if sampling_params_list is None else sampling_words(sampling_params_list, B, self._sampling_rng)
         if has_penalties(sampling_params_list):
             raise ValueError("forward_speculative does not apply penalties (their history is per position)")
+        if has_ngram_controls(sampling_params_list):
+            raise ValueError("forward_speculative does not apply no_repeat_ngram_size or DRY (their history is per position)")
         con = constraint_words(token_masks_list, sampling_params_list, B, self.model_config.vocab_size, rows=rows)
         slots = self._lora_slots(lora_ids_list, B, False)
         if B == 0:
@@ -663,9 +669,15 @@ class LlamaModel:
         samp = None if sampling_params_list is None else \
             sampling_words(sampling_params_list, len(input_ids_list), self._sampling_rng)
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
-        penalized = has_penalties(sampling_params_list)
+        ngram = has_ngram_controls(sampling_params_list)
+        penalized = ngram or has_penalties(sampling_params_list)
+        if ngram and ignore_kvcache:
+            raise ValueError("no_repeat_ngram_size and DRY need the token history of the block table: not available with "
+                             "ignore_kvcache")
         if penalized and ignore_kvcache:
             raise ValueError("penalties need the token history of the block table: not available with ignore_kvcache")
+        if ngram:
+            check_breaker_ids(sampling_params_list, self.model_config.vocab_size)
         if token_masks_list is not None and ignore_kvcache:
             raise ValueError("token_masks_list does not apply to the profiling forward (ignore_kvcache)")
         slots = self._lora_slots(lora_ids_list, len(input_ids_list), ignore_kvcache)
@@ -701,7 +713,7 @@ class LlamaModel:
             self.lora.ensure_rows(num_tokens)
         if graph:
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
-                                              top_n, penalized, sampled, con, slots)
+                                              top_n, penalized, sampled, con, slots, ngram)
         tiles = None if slots is None else lora_tiles(slots, prefill_lens + [1] * (batch_size - num_prefill_seqs))
 
         if not ignore_kvcache:
@@ -731,14 +743,16 @@ class LlamaModel:
 
     # ------------------------------------------------------------------ CUDA-graph decode path
     def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
-                              sampled=True, con: Optional[ConstraintWords] = None, slots: Optional[list] = None):
+                              sampled=True, con: Optional[ConstraintWords] = None, slots: Optional[list] = None,
+                              ngram: bool = False):
         """Pure-decode step replayed from a CUDA graph.  The step's metadata is staged through the same pinned ring as an eager
         step's, into the graph's static device buffer, and its blocks are reserved on the manager's host mirror like an eager
         step's; the graph (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
         allocation, gathers, every layer, lm_head and argmax - or, for sampled steps (`samp`: staged sampling words and the
         filtered flag, sampling_params.sampling_words), the sampling kernel, with the parameters staged in the same copy.  A step
         with log-probabilities (`top_n`) has its own graph, which also runs the log-probability kernel; so has a step with
-        penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples).  A
+        penalties, which also runs the penalty kernel (and the argmax instead of the sampling kernel when no row samples), and a
+        step with n-gram controls (`ngram`) the penalty kernel's n-gram launch, keyed by one more tag.  A
         constrained step (`con`: the graph-sized constraint region) has its own graph per bias capacity (the step's bias entries
         rounded up to a power of two), which also runs the constraint kernel.  An adapted step (`slots`, _lora_slots) has its own
         graph, which also runs the LoRA kernels over a tile list padded to B tiles, so any mix of slots replays it."""
@@ -758,7 +772,7 @@ class LlamaModel:
         if top_n is not None:
             key += ("logprobs", top_n)
         if penalized:
-            key += ("penalties", sampled)
+            key += ("penalties", sampled) + (("ngram",) if ngram else ())
         if con is not None:
             key += ("constrained", con.num_bias)
         if slots is not None:
@@ -772,7 +786,7 @@ class LlamaModel:
                 self._graphs.pop(next(iter(self._graphs)))
             g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled,
                                            None if con is None else con._replace(words=None),
-                                           **({} if slots is None else dict(lora=True)))
+                                           **({} if slots is None else dict(lora=True)), **(dict(ngram=True) if ngram else {}))
         self._graphs[key] = g                    # (re)insert as most recently used
         # the blocks are counted on the host, and the eager step's errors raised, before anything is enqueued; the graph's
         # allocation kernel hands them out
@@ -790,15 +804,16 @@ class LlamaModel:
 
     def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None,
                               penalized: bool = False, sampled: bool = True, con: Optional[ConstraintWords] = None,
-                              lora: bool = False):
+                              lora: bool = False, ngram: bool = False):
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
         also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
-        the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax.  con:
+        the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax.  ngram:
+        the meta starts with 28 * B words (the n-gram controls follow the penalties; all zero, so off, during the warm-up).  con:
         the sizes of the graph's constraint region (words None), which follows the sampling words; the graph constrains the
         logits first.  lora: B LoRA tiles follow (empty during the warm-up)."""
         ec = self.engine_config
         dev = self.device
-        nw = 0 if filtered is None else (8 if penalized else 5) * B
+        nw = 0 if filtered is None else (28 if ngram else 8 if penalized else 5) * B
         nc = 0 if con is None else ConstraintWords.size(*con[1:])
         nl = 3 * B if lora else 0
         meta = torch.zeros((nw + nc + nl + 3 * B,), dtype=torch.int32, device=dev)
