@@ -12,6 +12,7 @@ per generated token).  Needs an H100 (there is no CPU path).
     ... --prompt-logprobs 3    print each prompt's perplexity and the 3 most likely tokens at its first positions
     ... --repetition-penalty 1.1 --frequency-penalty 0.5 --presence-penalty 0.3    discourage repeats (vLLM's definitions)
     ... --no-repeat-ngram 3 / --dry-multiplier 0.8 [--dry-breakers 198 25]    ban repeated 3-grams / DRY phrase-repeat penalty
+    ... --temperature 1.0 --min-p 0.05 [--typical-p 0.9] [--xtc-threshold 0.1 --xtc-probability 0.5]    truncation filters
     ... --speculate 4      speculative decoding: verify up to 4 prompt-lookup drafts per step (forward_speculative)
     ... --n 4 --temperature 0.8    4 samples per prompt: each prompt is prefilled once and forked 3 times (fork_seqs)
     ... --lora /data/my-adapter    run every prompt under a PEFT LoRA adapter (load_lora, lora_ids_list)
@@ -167,6 +168,12 @@ def main():
     ap.add_argument("--dry-allowed-length", type=int, default=2, help="longest repeat DRY leaves alone")
     ap.add_argument("--dry-breakers", type=int, nargs="*", default=[],
                     help="DRY sequence-breaker token ids (the last token of encode('a' + s) for s in '\\n', ':', '\"', '*')")
+    ap.add_argument("--min-p", type=float, default=0.0, help="drop tokens less likely than min_p times the most likely one (0 = off)")
+    ap.add_argument("--typical-p", type=float, default=1.0,
+                    help="keep the tokens nearest the entropy that carry this much mass (typical sampling; 1 = off)")
+    ap.add_argument("--xtc-threshold", type=float, default=0.1, help="XTC: tokens at least this likely are top choices")
+    ap.add_argument("--xtc-probability", type=float, default=0.0,
+                    help="XTC: chance per step of removing every top choice but the least likely one (0 = off)")
     ap.add_argument("--speculate", type=int, default=0, help="verify up to K (<= 7) prompt-lookup drafts per decode step (0 = off)")
     ap.add_argument("--n", type=int, default=1, help="samples per prompt: prefill once, fork n - 1 times, distinct seeds (1 = off)")
     ap.add_argument("--lora", type=str, default=None, help="PEFT LoRA adapter directory: every prompt runs under this adapter")
@@ -222,7 +229,9 @@ def main():
                                           presence_penalty=args.presence_penalty, no_repeat_ngram_size=args.no_repeat_ngram,
                                           dry_multiplier=args.dry_multiplier, dry_base=args.dry_base,
                                           dry_allowed_length=args.dry_allowed_length,
-                                          dry_sequence_breakers=tuple(args.dry_breakers))
+                                          dry_sequence_breakers=tuple(args.dry_breakers), min_p=args.min_p,
+                                          typical_p=args.typical_p, xtc_threshold=args.xtc_threshold,
+                                          xtc_probability=args.xtc_probability)
     if (args.temperature == 0 and args.logprobs is None and args.prompt_logprobs is None and not params.has_penalties()
             and not params.has_ngram_controls()):
         params = None

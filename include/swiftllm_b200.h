@@ -283,6 +283,22 @@ int sllm_sample_tokens(const void* logits, int64_t num_rows, int vocab_size, int
                        const int64_t* seed, const int32_t* pos, int64_t* out_tokens, float* out_pairs, sllm_dtype_t dtype,
                        sllm_stream_t stream);
 
+/* ---- Truncation filters (new): sllm_sample_tokens with the per-row DEVICE arrays [num_rows] min_p (0: off), typical_p (>= 1:
+ * off), xtc_threshold and xtc_probability (0: off), applied in this order after min-p: top-k, top-p, typical-p, XTC.  With
+ * x = (m - l) / T, q = expf(-x) and w = round(q * 2^40) over the survivors of the previous filter (Z their exact sum):
+ * min-p keeps key >= the smallest key with q >= min_p (before top-k and top-p); typical-p keeps |x - c| <= delta, c =
+ * fp32(E / Z) with E = sum round(fp32(q * x) * 2^40), delta the smallest distance whose survivors weigh >= typical_p * Z; XTC,
+ * when u = Philox(seed, counter (0, pos, 1, 0)) word 0 drawn as the Gumbel noise's u is < xtc_probability and at least two
+ * finite survivors have w >= xtc_threshold * Z, drops the survivors above the smallest key among those (its ties kept; a
+ * -inf id is never counted, so threshold 0 stops at the least likely finite survivor).  Every kept
+ * set is a key interval; greedy and bad rows, the draw and out_pairs are those of sllm_sample_tokens, and with every filter
+ * off the result is its result.  Rejected before launch: what sllm_sample_tokens rejects, and null filter arrays. */
+int sllm_sample_tokens_truncated(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                                 int64_t vocab_offset, const float* temperature, const int32_t* top_k, const float* top_p,
+                                 const int64_t* seed, const int32_t* pos, int64_t* out_tokens, float* out_pairs,
+                                 const float* min_p, const float* typical_p, const float* xtc_threshold,
+                                 const float* xtc_probability, sllm_dtype_t dtype, sllm_stream_t stream);
+
 /* ---- Token log-probabilities (new; the reference returns token ids only): log_softmax of the raw 16-bit logits (no
  * temperature, no top-k / top-p), logits as in sllm_sample_tokens with the whole vocabulary in each row.
  * m = the largest logit, Z = sum_v round(expf(l_v - m) * 2^40) as an exact 64-bit integer, lse = m + logf(Z * 2^-40) and

@@ -52,6 +52,7 @@ SIGNATURES = {
     "sllm_swap_blocks": (_I, [_P, _P, _L, _I, _P, _P, _P, _P, _L, _P]),
     "sllm_swap_blocks_gathered": (_I, [_P, _P, _L, _I, _P, _P, _P, _P, _L, _P]),
     "sllm_sample_tokens": (_I, [_P, _L, _I, _L, _L, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "sllm_sample_tokens_truncated": (_I, [_P, _L, _I, _L, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
     "sllm_token_logprobs": (_I, [_P, _L, _I, _L, _P, _I, _P, _P, _P, _I, _P]),
     "sllm_prompt_logprobs": (_I, [_P, _L, _I, _L, _P, _I, _P, _P, _P, _P, _I, _P]),
     "sllm_apply_penalties": (_I, [_P, _L, _I, _L, _L, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _L, _I, _P]),

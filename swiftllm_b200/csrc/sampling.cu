@@ -50,12 +50,56 @@ __device__ __forceinline__ bool better(float s, int64_t i, float bs, int64_t bi)
     return s > bs || (s == bs && i < bi);
 }
 
-template <typename T>
+// The per-row filter arrays of the kTrunc instantiation (sllm_sample_tokens_truncated), passed after the other parameters so
+// that theirs keep their offsets; the plain instantiation gets null pointers and never reads them.
+struct TruncRows {
+    const float* min_p;
+    const float* typical_p;
+    const float* xtc_threshold;
+    const float* xtc_probability;
+};
+
+// The cluster's (smallest key, largest key, sum of w, sum of e) over the staged keys for which in(key) holds, acc(key, w, e)
+// adding that key's terms.  Each CTA posts its part in `slot` (4 words of its shared memory, written once per kernel) and every
+// thread reads all of them: a pure function of the row, whatever the cluster size.  Block-wide; ends with a cluster barrier.
+struct Span { uint32_t lo, hi; unsigned long long w, e; };
+template <typename In, typename Acc>
+__device__ __forceinline__ Span cluster_span(cg::cluster_group& cluster, const uint16_t* keys, int n, unsigned long long* slot,
+                                             unsigned long long* scratch, In&& in, Acc&& acc) {
+    uint32_t lo = 0xffffffffu, hi = 0;
+    unsigned long long w = 0, e = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const uint32_t key = keys[i];
+        if (in(key)) {
+            lo = min(lo, key);
+            hi = max(hi, key);
+            acc(key, w, e);
+        }
+    }
+    lo = block_min_u32(lo, scratch);
+    hi = (uint32_t)block_max_u64(hi, scratch);
+    w = block_sum_u64(w, scratch);
+    e = block_sum_u64(e, scratch);
+    if (threadIdx.x == 0) { slot[0] = lo; slot[1] = hi; slot[2] = w; slot[3] = e; }
+    cluster.sync();
+    Span s{0xffffffffu, 0u, 0ull, 0ull};
+    for (unsigned r = 0; r < cluster.num_blocks(); r++) {
+        const unsigned long long* p = cluster.map_shared_rank(slot, r);
+        s.lo = min(s.lo, (uint32_t)p[0]);
+        s.hi = max(s.hi, (uint32_t)p[1]);
+        s.w += p[2];
+        s.e += p[3];
+    }
+    return s;
+}
+
+template <typename T, bool kTrunc>
 __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ logits, int64_t row_stride, int V,
                                                           int64_t vocab_offset, int slice, const float* __restrict__ temperature,
                                                           const int32_t* __restrict__ top_k, const float* __restrict__ top_p,
                                                           const int64_t* __restrict__ seed, const int32_t* __restrict__ pos,
-                                                          int64_t* __restrict__ out_tokens, float* __restrict__ out_pairs) {
+                                                          int64_t* __restrict__ out_tokens, float* __restrict__ out_pairs,
+                                                          TruncRows tr) {
     extern __shared__ uint16_t keys[];
     __shared__ unsigned long long h_cnt_hi[256], h_cnt_lo[256], h_mass_hi[256], h_mass_lo[256], merged[256];
     __shared__ unsigned long long scratch[32];
@@ -75,6 +119,10 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
 
     // ---- stage the slice as keys; local (max key, smallest index)
     for (int i = threadIdx.x; i < 256; i += blockDim.x) h_cnt_hi[i] = h_cnt_lo[i] = h_mass_hi[i] = h_mass_lo[i] = 0;
+    // kTrunc: the four byte histograms of the typical-p select and the per-stage cluster_span slots
+    __shared__ unsigned long long h_dist[kTrunc ? 4 * 256 : 1], span_slot[kTrunc ? 4 * 4 : 1];
+    if constexpr (kTrunc)
+        for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x) h_dist[i] = 0;
     unsigned long long best = 0;
     bool bad = false;                                                 // a NaN of either sign or +inf
     stage_keys(reinterpret_cast<const uint16_t*>(src), n, keys, [&](uint32_t k, int i) {
@@ -105,8 +153,20 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
         return;
     }
 
-    // ---- top-k threshold
+    // ---- kTrunc: min-p, keep key >= the smallest key with q >= min_p (the maximum has q = 1, so some key passes)
     uint32_t thr = 0;
+    const float m_row = value_of<T>(max_key);
+    if constexpr (kTrunc) {
+        const float mp = tr.min_p[row];
+        if (mp > 0.f)
+            thr = cluster_span(cluster, keys, n, span_slot, scratch,
+                               [&](uint32_t key) { return expf(__fdiv_rn(__fsub_rn(value_of<T>(key), m_row), temp)) >= mp; },
+                               [](uint32_t, unsigned long long&, unsigned long long&) {}).lo;
+    }
+    const uint32_t thr_min_p = thr;
+    thr = 0;
+
+    // ---- top-k threshold
     const int k = top_k[row];
     if (k > 0 && k < V) {
         for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
@@ -120,6 +180,8 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
         thr = select_low_byte(cluster, keys, n, (uint32_t)sel_bin, above, merged, h_cnt_lo, (double)k,
                               [](uint32_t) { return true; }, [](uint32_t, bool) { return 1ull; }, &sel_bin, &sel_above).tau;
     }
+
+    if constexpr (kTrunc) thr = thr_min_p > thr ? thr_min_p : thr;
 
     // ---- top-p threshold over the survivors
     const float p = top_p[row];
@@ -154,6 +216,60 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
         thr = tp > thr ? tp : thr;
     }
 
+    // ---- kTrunc: typical-p and XTC over the survivors [thr, hi]; every kept set stays a key interval
+    uint32_t hi = 0xffffu;
+    if constexpr (kTrunc) {
+        // x = (m - l) / T, q = expf(-x) (bit for bit the top-p q), w = round(q * 2^40), e = round(q * x * 2^40) (0 when w is)
+        auto x_of = [&](uint32_t key) { return __fdiv_rn(__fsub_rn(m_row, value_of<T>(key)), temp); };
+        auto w_of = [](float x) { return (unsigned long long)__float2ull_rn(__fmul_rn(expf(-x), kMassScale)); };
+        auto alive = [&](uint32_t key) { return key >= thr && key <= hi; };
+        auto add_w = [&](uint32_t key, unsigned long long& w, unsigned long long&) { w += w_of(x_of(key)); };
+        const float typ = tr.typical_p[row];
+        unsigned long long Z = 0;
+        bool have_z = false;
+        if (typ < 1.f) {
+            const Span s = cluster_span(cluster, keys, n, span_slot + 4, scratch, alive,
+                                        [&](uint32_t key, unsigned long long& w, unsigned long long& e) {
+                                            const float x = x_of(key);
+                                            const float q = expf(-x);
+                                            const unsigned long long wk = __float2ull_rn(__fmul_rn(q, kMassScale));
+                                            w += wk;
+                                            if (wk) e += __float2ull_rn(__fmul_rn(__fmul_rn(q, x), kMassScale));
+                                        });
+            const float c = (float)((double)s.e / (double)s.w);
+            auto d_bits = [&](uint32_t key) { return __float_as_uint(fabsf(__fsub_rn(x_of(key), c))); };
+            // delta: the smallest distance whose survivors with d <= delta weigh >= typical_p * Z (order ~bits: small d first)
+            const uint32_t u = select_u32(cluster, keys, n, h_dist, merged, (double)typ * (double)s.w, alive,
+                                          [&](uint32_t key) { return ~d_bits(key); },
+                                          [&](uint32_t key) { return w_of(x_of(key)); }, &sel_bin, &sel_above);
+            const uint32_t delta = ~u;
+            const Span k = cluster_span(cluster, keys, n, span_slot + 8, scratch,
+                                        [&](uint32_t key) { return alive(key) && d_bits(key) <= delta; }, add_w);
+            thr = k.lo;
+            hi = k.hi;
+            Z = k.w;
+            have_z = true;
+        }
+        const float xp = tr.xtc_probability[row];
+        if (xp > 0.f) {
+            const uint64_t sd = (uint64_t)seed[row];
+            const uint4 r = philox4x32_10(make_uint4(0u, (uint32_t)pos[row], 1u, 0u), (uint32_t)sd, (uint32_t)(sd >> 32));
+            if (__fmul_rn((float)(r.x >> 9) + 0.5f, 1.0f / 8388608.0f) < xp) {
+                if (!have_z) Z = cluster_span(cluster, keys, n, span_slot + 8, scratch, alive, add_w).w;
+                const double bar = (double)tr.xtc_threshold[row] * (double)Z;
+                // the top choices, the finite survivors whose w reaches threshold * Z, are the survivors from some key up: their
+                // count and smallest key.  A -inf id (masked, banned) is never one, so threshold 0 stops at the least likely
+                // finite survivor and the draw can never pick a -inf id over it.
+                const Span t = cluster_span(cluster, keys, n, span_slot + 12, scratch,
+                                            [&](uint32_t key) {
+                                                return alive(key) && key > InfKeys<T>::neg && (double)w_of(x_of(key)) >= bar;
+                                            },
+                                            [](uint32_t, unsigned long long& w, unsigned long long&) { w += 1; });
+                if (t.w >= 2) hi = t.lo;
+            }
+        }
+    }
+
     // ---- Gumbel-max over the kept tokens; the noise of 4 consecutive GLOBAL indices comes from one Philox call
     const uint64_t sd = (uint64_t)seed[row];
     const uint32_t k0 = (uint32_t)sd, k1 = (uint32_t)(sd >> 32), ctr_pos = (uint32_t)pos[row];
@@ -168,7 +284,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
             for (int j = 0; j < 4; j++) {
                 const int64_t lv = 4 * g + j - vocab_offset - begin;
                 const uint32_t key = (lv >= 0 && lv < n) ? keys[lv] : 0u;
-                kk[j] = (lv >= 0 && lv < n && key >= thr) ? key : 0xffffffffu;       // 0xffffffff: not kept
+                kk[j] = (lv >= 0 && lv < n && key >= thr && (!kTrunc || key <= hi)) ? key : 0xffffffffu;   // 0xffffffff: not kept
                 any |= kk[j] != 0xffffffffu;
             }
             if (!any) continue;
@@ -213,25 +329,57 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
 }  // namespace
 }  // namespace sllm
 
+namespace sllm {
+namespace {
+
+// The argument checks and the launch of both entry points; `truncated` selects the kTrunc instantiation.
+int sample_tokens(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride, int64_t vocab_offset,
+                  const float* temperature, const int32_t* top_k, const float* top_p, const int64_t* seed, const int32_t* pos,
+                  int64_t* out_tokens, float* out_pairs, bool truncated, TruncRows tr, sllm_dtype_t dtype, cudaStream_t stream,
+                  const char* name) {
+    SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "%s: unsupported dtype tag %d", name, (int)dtype);
+    SLLM_REQUIRE(num_rows >= 0 && num_rows <= (1 << 20), "%s: num_rows %lld out of range", name, (long long)num_rows);
+    SLLM_REQUIRE(vocab_size > 0, "%s: vocab_size must be positive, got %d", name, vocab_size);
+    SLLM_REQUIRE(slice_fits(vocab_size, kMaxCluster, kKeyBytes, kKeyAlign),
+                 "%s: vocab_size %d does not fit the shared memory of a %d-CTA cluster", name, vocab_size, kMaxCluster);
+    SLLM_REQUIRE(vocab_offset >= 0 && vocab_offset + vocab_size <= (1 << 24),
+                 "%s: global vocabulary indices must stay below 2^24 (vocab_offset %lld)", name, (long long)vocab_offset);
+    SLLM_REQUIRE(logits_row_stride >= vocab_size, "%s: logits_row_stride %lld < vocab_size %d", name,
+                 (long long)logits_row_stride, vocab_size);
+    if (num_rows == 0) return 0;
+    SLLM_REQUIRE(logits && temperature && top_k && top_p && seed && pos && out_tokens, "%s: null pointer", name);
+    SLLM_REQUIRE(!truncated || (tr.min_p && tr.typical_p && tr.xtc_threshold && tr.xtc_probability),
+                 "%s: null filter array", name);
+    const ClusterGeometry g = cluster_geometry(num_rows, vocab_size, kKeyBytes, kKeyAlign);
+    const size_t smem = (size_t)g.slice * kKeyBytes;
+    if (truncated)
+        SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<sample_kernel<T, true>>(
+                                       num_rows, g.C, smem, stream, name, (const T*)logits, logits_row_stride, vocab_size,
+                                       vocab_offset, g.slice, temperature, top_k, top_p, seed, pos, out_tokens, out_pairs, tr));
+    SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<sample_kernel<T, false>>(
+                                   num_rows, g.C, smem, stream, name, (const T*)logits,
+                                   logits_row_stride, vocab_size, vocab_offset, g.slice, temperature, top_k, top_p, seed, pos,
+                                   out_tokens, out_pairs, tr));
+}
+
+}  // namespace
+}  // namespace sllm
+
 extern "C" int sllm_sample_tokens(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
                                   int64_t vocab_offset, const float* temperature, const int32_t* top_k, const float* top_p,
                                   const int64_t* seed, const int32_t* pos, int64_t* out_tokens, float* out_pairs,
                                   sllm_dtype_t dtype, sllm_stream_t stream) {
-    using namespace sllm;
-    SLLM_REQUIRE(dtype == SLLM_F16 || dtype == SLLM_BF16, "sample_tokens: unsupported dtype tag %d", (int)dtype);
-    SLLM_REQUIRE(num_rows >= 0 && num_rows <= (1 << 20), "sample_tokens: num_rows %lld out of range", (long long)num_rows);
-    SLLM_REQUIRE(vocab_size > 0, "sample_tokens: vocab_size must be positive, got %d", vocab_size);
-    SLLM_REQUIRE(slice_fits(vocab_size, kMaxCluster, kKeyBytes, kKeyAlign),
-                 "sample_tokens: vocab_size %d does not fit the shared memory of a %d-CTA cluster", vocab_size, kMaxCluster);
-    SLLM_REQUIRE(vocab_offset >= 0 && vocab_offset + vocab_size <= (1 << 24),
-                 "sample_tokens: global vocabulary indices must stay below 2^24 (vocab_offset %lld)", (long long)vocab_offset);
-    SLLM_REQUIRE(logits_row_stride >= vocab_size, "sample_tokens: logits_row_stride %lld < vocab_size %d",
-                 (long long)logits_row_stride, vocab_size);
-    if (num_rows == 0) return 0;
-    SLLM_REQUIRE(logits && temperature && top_k && top_p && seed && pos && out_tokens, "sample_tokens: null pointer");
-    const ClusterGeometry g = cluster_geometry(num_rows, vocab_size, kKeyBytes, kKeyAlign);
-    SLLM_DISPATCH_DTYPE(dtype, return launch_cluster<sample_kernel<T>>(
-                                   num_rows, g.C, (size_t)g.slice * kKeyBytes, (cudaStream_t)stream, "sample_tokens",
-                                   (const T*)logits, logits_row_stride, vocab_size, vocab_offset, g.slice, temperature, top_k,
-                                   top_p, seed, pos, out_tokens, out_pairs));
+    return sllm::sample_tokens(logits, num_rows, vocab_size, logits_row_stride, vocab_offset, temperature, top_k, top_p, seed,
+                               pos, out_tokens, out_pairs, false, sllm::TruncRows{}, dtype, (cudaStream_t)stream, "sample_tokens");
+}
+
+extern "C" int sllm_sample_tokens_truncated(const void* logits, int64_t num_rows, int vocab_size, int64_t logits_row_stride,
+                                            int64_t vocab_offset, const float* temperature, const int32_t* top_k,
+                                            const float* top_p, const int64_t* seed, const int32_t* pos, int64_t* out_tokens,
+                                            float* out_pairs, const float* min_p, const float* typical_p,
+                                            const float* xtc_threshold, const float* xtc_probability, sllm_dtype_t dtype,
+                                            sllm_stream_t stream) {
+    return sllm::sample_tokens(logits, num_rows, vocab_size, logits_row_stride, vocab_offset, temperature, top_k, top_p, seed,
+                               pos, out_tokens, out_pairs, true, sllm::TruncRows{min_p, typical_p, xtc_threshold, xtc_probability},
+                               dtype, (cudaStream_t)stream, "sample_tokens_truncated");
 }

@@ -239,6 +239,42 @@ __device__ __forceinline__ Selected select_low_byte(cg::cluster_group& cluster, 
     return {(hi << 8) | (uint32_t)*sel_bin, *sel_above};
 }
 
+// The four-byte form of the same select over a 32-bit order of the keys: the largest u such that the weight of the counted
+// keys with order(key) >= u reaches `target` (one histogram, DSMEM merge and select_bin per byte, high byte first).  order(key)
+// is called for every staged key and only read where counts(key) holds; weight(key) where the key counts and matches the bytes
+// chosen so far.  h: this CTA's four zeroed 256-bin histograms (h[256 * j] for byte 3 - j), used once each.  Block-wide; the
+// caller guarantees the target is reached (it is at most the total weight).
+template <typename Counts, typename Order, typename Weight>
+__device__ __forceinline__ uint32_t select_u32(cg::cluster_group& cluster, const uint16_t* keys, int n,
+                                               unsigned long long* h, unsigned long long* merged, double target,
+                                               Counts&& counts, Order&& order, Weight&& weight, int* sel_bin,
+                                               unsigned long long* sel_above) {
+    uint32_t prefix = 0;
+    unsigned long long above = 0;
+#pragma unroll 1
+    for (int j = 0; j < 4; j++) {
+        const int sh = 24 - 8 * j;
+        for (int i0 = threadIdx.x & ~31; i0 < n; i0 += blockDim.x) {
+            const int i = i0 + (threadIdx.x & 31);
+            const uint32_t key = i < n ? keys[i] : 0u;
+            const bool c = i < n && counts(key);
+            const uint32_t o = c ? order(key) : 0u;
+            const bool in = c && (uint32_t)((unsigned long long)o >> (sh + 8)) == prefix;
+            warp_hist_add(h + 256 * j, in, (o >> sh) & 255u, in ? weight(key) : 0ull);
+        }
+        merge_hist(cluster, h + 256 * j, merged);
+        select_bin(merged, above, target, sel_bin, sel_above);
+        prefix = (prefix << 8) | (uint32_t)*sel_bin;
+        above = *sel_above;
+    }
+    return prefix;
+}
+
+// Block-wide min of a uint32 (all threads get it), through block_max_u64.
+__device__ __forceinline__ uint32_t block_min_u32(uint32_t v, unsigned long long* scratch) {
+    return 0xffffffffu - (uint32_t)block_max_u64(0xffffffffu - v, scratch);
+}
+
 // ---------------------------------------------------------------- host: one thread-block cluster of C CTAs per row
 
 // Whether a row of V entries split over c CTAs, each slice rounded up to `align` entries, fits kMaxSliceBytes per CTA.

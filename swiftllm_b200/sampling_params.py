@@ -52,7 +52,19 @@ class SamplingParams:
     each string s of ["\n", ":", "\"", "*"], the last token id of tokenizer.encode("a" + s).
     The order per token is: penalties, DRY, ban, one rounding to the storage dtype; they run after the mask and logit_bias.  A
     row whose mask and bans leave no token allowed gets the all -inf row rule of the token choice.  Log-probabilities stay those
-    of the raw logits.  forward_speculative and ignore_kvcache raise ValueError for them, as for the penalties."""
+    of the raw logits.  forward_speculative and ignore_kvcache raise ValueError for them, as for the penalties.
+
+    Truncation filters (csrc/sampling.cu, sllm_sample_tokens_truncated), for rows with temperature > 0 (greedy rows ignore them,
+    as they ignore top_k / top_p).  With q_v = exp((l_v - m) / T) (m the row's largest logit) over the tokens the previous filter
+    kept, in this order: min_p (0: off) keeps q_v >= min_p (vLLM's p_v >= min_p * p_max), before top-k and top-p, so top-p's mass
+    is taken over the min-p survivors; then top_k and top_p; then typical_p (1: off), Hugging Face's typical sampling, keeps the
+    tokens whose surprisal -log p_v is nearest the entropy H, the fewest (by distance) whose probability reaches typical_p; then
+    XTC ("exclude top choices", llama.cpp / text-generation-webui): with probability xtc_probability (0: off), when at least two
+    tokens have p_v >= xtc_threshold, every token above the least likely of those is removed (a masked or banned token is never
+    one of them, so xtc_threshold 0 keeps the least likely allowed token).  Tokens tied with the last one kept
+    by any filter are kept; so XTC keeps every token tied with that least likely top choice, where llama.cpp keeps one of them.
+    The XTC draw is seeded like the token (seed, sequence length), from its own noise stream.  Log-probabilities stay those of
+    the raw logits."""
     temperature: float = 0.0
     top_k: int = 0
     top_p: float = 1.0
@@ -68,6 +80,10 @@ class SamplingParams:
     dry_base: float = 1.75
     dry_allowed_length: int = 2
     dry_sequence_breakers: tuple = ()
+    min_p: float = 0.0
+    typical_p: float = 1.0
+    xtc_threshold: float = 0.1
+    xtc_probability: float = 0.0
 
     def validate(self):
         if not (isinstance(self.temperature, (int, float)) and math.isfinite(self.temperature) and self.temperature >= 0):
@@ -118,6 +134,12 @@ class SamplingParams:
                 raise ValueError(f"dry_sequence_breakers must hold token ids (integers >= 0), got {t!r}")
         if len(set(int(t) for t in br)) != len(br):
             raise ValueError(f"dry_sequence_breakers ids must be distinct, got {tuple(br)!r}")
+        for name in ("min_p", "xtc_threshold", "xtc_probability"):
+            v = getattr(self, name)
+            if not (_is_real(v) and math.isfinite(v) and 0 <= v <= 1):
+                raise ValueError(f"{name} must be a finite number in [0, 1], got {v!r}")
+        if not (_is_real(self.typical_p) and math.isfinite(self.typical_p) and 0 < self.typical_p <= 1):
+            raise ValueError(f"typical_p must be a finite number in (0, 1], got {self.typical_p!r}")
 
     def has_penalties(self) -> bool:
         return self.repetition_penalty != 1.0 or self.frequency_penalty != 0.0 or self.presence_penalty != 0.0
@@ -125,6 +147,10 @@ class SamplingParams:
     def has_ngram_controls(self) -> bool:
         """The no-repeat n-gram ban or DRY is on."""
         return self.no_repeat_ngram_size > 0 or self.dry_multiplier > 0
+
+    def has_truncation(self) -> bool:
+        """min-p, typical-p or XTC is on (they apply to rows with temperature > 0)."""
+        return self.min_p > 0 or self.typical_p < 1 or self.xtc_probability > 0
 
 
 def _is_real(v) -> bool:
@@ -176,8 +202,10 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
     """Validates the list and returns the staged int32 words (seed lo/hi interleaved [2B], temperature bits [B], top_k [B],
     top_p bits [B], and when some row has penalties or n-gram controls the fp32 bits of repetition, frequency and presence
     penalty [3B]; when some row has n-gram controls then no_repeat_ngram_size [B], dry_allowed_length [B], the fp32 bits of
-    dry_multiplier [B] and dry_base [B], and dry_sequence_breakers [B, 16] padded with -1) and whether any row filters (top-k /
-    top-p); None when every row is greedy and none has penalties or n-gram controls.  Raises ValueError."""
+    dry_multiplier [B] and dry_base [B], and dry_sequence_breakers [B, 16] padded with -1; when some row samples with min-p,
+    typical-p or XTC (has_truncation) then, last, the fp32 bits of min_p [B], typical_p [B], xtc_threshold [B] and
+    xtc_probability [B]) and whether any row filters (top-k / top-p / those three); None when every row is greedy and none has
+    penalties or n-gram controls.  Raises ValueError."""
     if len(params_list) != batch_size:
         raise ValueError(f"sampling_params_list has {len(params_list)} entries for a batch of {batch_size}")
     for sp in params_list:
@@ -193,7 +221,7 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
     temp = np.array([sp.temperature for sp in params_list], dtype=np.float32)
     top_p = np.array([sp.top_p for sp in params_list], dtype=np.float32)
     top_k = [int(sp.top_k) for sp in params_list]
-    filtered = any(sp.temperature > 0 and (sp.top_k > 0 or sp.top_p < 1) for sp in params_list)
+    filtered = any(sp.temperature > 0 and (sp.top_k > 0 or sp.top_p < 1 or sp.has_truncation()) for sp in params_list)
     words = _i32(seeds.view(np.uint32)) + _i32(temp.view(np.uint32)) + top_k + _i32(top_p.view(np.uint32))
     if penalized:
         for name in ("repetition_penalty", "frequency_penalty", "presence_penalty"):
@@ -205,7 +233,19 @@ def sampling_words(params_list: list, batch_size: int, rng: np.random.Generator)
         for sp in params_list:
             br = [int(t) for t in sp.dry_sequence_breakers]
             words += br + [-1] * (MAX_DRY_BREAKERS - len(br))
+    if has_truncation(params_list):
+        for name in TRUNCATION_FIELDS:
+            words += _i32(np.array([getattr(sp, name) for sp in params_list], dtype=np.float32).view(np.uint32))
     return words, filtered
+
+
+TRUNCATION_FIELDS = ("min_p", "typical_p", "xtc_threshold", "xtc_probability")
+
+
+def has_truncation(params_list: Optional[list]) -> bool:
+    """Some entry of the (validated) list samples (temperature > 0) with min-p, typical-p or XTC: its sampling words end with
+    the 4 * B filter words and the token comes from sllm_sample_tokens_truncated."""
+    return any(sp.temperature > 0 and sp.has_truncation() for sp in params_list or [])
 
 
 def has_penalties(params_list: Optional[list]) -> bool:

@@ -104,6 +104,11 @@ class SamplingState:
     dry_multiplier: Optional[torch.Tensor] = None           # [batch_size] float32, 0 = off
     dry_base: Optional[torch.Tensor] = None                 # [batch_size] float32
     dry_breakers: Optional[torch.Tensor] = None             # [batch_size, 16] int32, -1 = unused
+    # ---- min-p, typical-p and XTC (csrc/sampling.cu, the truncated entry); None when no sampled row of the step has them
+    min_p: Optional[torch.Tensor] = None                    # [batch_size] float32, 0 = off
+    typical_p: Optional[torch.Tensor] = None                # [batch_size] float32, 1 = off
+    xtc_threshold: Optional[torch.Tensor] = None            # [batch_size] float32
+    xtc_probability: Optional[torch.Tensor] = None          # [batch_size] float32, 0 = off
     sampled: bool = True            # some row has temperature > 0; False: every row takes the argmax of its penalised logits
     # the token history the penalty kernel reads and extends, set by the model: the step's input ids (int32 [num_tokens]), the
     # block table and the token pages (int32 [num_blocks, block_size])
@@ -119,6 +124,17 @@ class SamplingState:
     def ngram(self) -> bool:
         return self.no_repeat_ngram_size is not None
 
+    @property
+    def truncated(self) -> bool:
+        return self.min_p is not None
+
+    def truncation_kwargs(self) -> dict:
+        """The filter keyword arguments of worker.kernels.sampling.sample_tokens ({} without them)."""
+        if not self.truncated:
+            return {}
+        return dict(min_p=self.min_p, typical_p=self.typical_p, xtc_threshold=self.xtc_threshold,
+                    xtc_probability=self.xtc_probability)
+
     def ngram_kwargs(self) -> dict:
         """The n-gram keyword arguments of worker.kernels.penalties.apply_penalties ({} without n-gram controls)."""
         if not self.ngram:
@@ -127,13 +143,19 @@ class SamplingState:
                     dry_multiplier=self.dry_multiplier, dry_base=self.dry_base, dry_breakers=self.dry_breakers)
 
     @staticmethod
-    def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool, sampled: bool = True) -> "SamplingState":
+    def from_staged(words: torch.Tensor, pos: torch.Tensor, filtered: bool, sampled: bool = True,
+                    truncated: bool = False) -> "SamplingState":
         """`words`: the int32 device view staged from swiftllm_b200.sampling_params.sampling_words (8-byte aligned); 8 * B
-        words carry the penalties after the 5 * B sampling words; 28 * B words also the n-gram controls after those."""
+        words carry the penalties after the 5 * B sampling words; 28 * B words also the n-gram controls after those.
+        `truncated` (sampling_params.has_truncation): the last 4 * B words are the min-p, typical-p and XTC parameters."""
         B = pos.shape[0]
         pen = {}
+        if truncated:
+            t = words[words.shape[0] - 4 * B:].view(torch.float32)
+            pen = dict(min_p=t[:B], typical_p=t[B:2 * B], xtc_threshold=t[2 * B:3 * B], xtc_probability=t[3 * B:])
+            words = words[:words.shape[0] - 4 * B]
         if words.shape[0] in (8 * B, 28 * B):
-            pen = dict(repetition_penalty=words[5 * B:6 * B].view(torch.float32),
+            pen.update(repetition_penalty=words[5 * B:6 * B].view(torch.float32),
                        frequency_penalty=words[6 * B:7 * B].view(torch.float32),
                        presence_penalty=words[7 * B:8 * B].view(torch.float32))
         if words.shape[0] == 28 * B:

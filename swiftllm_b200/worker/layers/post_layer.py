@@ -30,7 +30,10 @@ Addition (constrained decoding, csrc/constraints.cu): when some row carries an a
 (infer_state.constraints), the logits the token is chosen from are masked and biased first, ahead of the penalties (a copy when
 log-probabilities are asked for: they stay those of the raw logits).  With a sharded lm_head the pair-merge path constrains each
 rank's shard (vocab_offset) before its local choice - a shard with no allowed id yields a -inf pair, which the merge never picks
-because the host checked that every mask allows some id; the gather path constrains the gathered full rows on every rank."""
+because the host checked that every mask allows some id; the gather path constrains the gathered full rows on every rank.
+
+Addition (min-p, typical-p and XTC, csrc/sampling.cu): rows with these filters (sampling.truncated) are sampled by the truncated
+entry with their filter views.  The filters need whole rows, so such rows count as filtered and a sharded lm_head gathers them."""
 import torch
 import torch.distributed as dist
 
@@ -127,7 +130,7 @@ class LlamaPostLayer:
             if pen:
                 chosen = self._penalised(chosen, infer_state, idx, copy=n is not None and con is None)
             if sampled:
-                tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos)
+                tokens = sample_tokens(chosen, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos, **sp.truncation_kwargs())
             else:
                 tokens = torch.argmax(chosen, dim=1)
             return tokens if n is None else (tokens,) + token_logprobs(full, tokens, n)
@@ -139,7 +142,7 @@ class LlamaPostLayer:
         if sampled:
             mine = torch.empty((B, 2), dtype=torch.float32, device=logits.device)
             sample_tokens(logits, sp.temperature, sp.top_k, sp.top_p, sp.seed, sp.pos, vocab_offset=self.tp_rank * Vs,
-                          out_pairs=mine)
+                          out_pairs=mine, **sp.truncation_kwargs())
         else:
             local = torch.argmax(logits, dim=1)
             mine = torch.stack((logits.gather(1, local[:, None]).squeeze(1).float(),

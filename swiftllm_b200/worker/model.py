@@ -35,7 +35,7 @@ from swiftllm_b200 import swiftllm_c
 from swiftllm_b200.engine_config import EngineConfig
 from swiftllm_b200.model_config import LlamaModelConfig
 from swiftllm_b200.sampling_params import (ConstraintWords, PromptLogprobs, SamplingParams, TokenLogprobs, constraint_words,
-                                           check_breaker_ids, has_ngram_controls, has_penalties, logprobs_top_n,
+                                           check_breaker_ids, has_ngram_controls, has_penalties, has_truncation, logprobs_top_n,
                                            prompt_logprobs_top_n, sampling_words)
 from swiftllm_b200.utils import GB
 from swiftllm_b200.worker import fp8 as fp8_weights
@@ -379,13 +379,13 @@ class LlamaModel:
                      decoding_lens: Optional[list], prefix=None, max_prefill_kv_len: int = 0, speculative: bool = False,
                      ignore_kvcache: bool = False, words=None, filtered: bool = False, sampled: bool = True, sampling_pos=None,
                      top_n: Optional[int] = None, prompt_state: Optional[PromptLogprobsState] = None, block_table=None,
-                     token_cache=None, constraints=None, lora_tiles_view=None) -> LlamaInferState:
+                     token_cache=None, constraints=None, lora_tiles_view=None, truncated: bool = False) -> LlamaInferState:
         """The LlamaInferState of a step from its int32 device views (input ids, block-table rows, sequence lengths with the
         prefill entries first, prompt lengths and first rows, positions, rows to sample) and the sizes the host knows; the batch
         counts are the views' shapes.  decoding_lens: host decode lengths for the reference's split heuristic, None in a graph
         captured for a length bucket (the largest split).  prefix: first position of each chunk (chunked prefill, speculative
         verification), with max_prefill_kv_len.  words: staged sampling_params.sampling_words, noise counter `sampling_pos`
-        (default: the sequence lengths); with penalties the sampling state also carries the token history: the input ids, the
+        (default: the sequence lengths), ending with the min-p / typical-p / XTC words when `truncated`; with penalties the sampling state also carries the token history: the input ids, the
         block table and the token pages (default: the model's).  constraints: (device view of the staged constraint region, its
         sampling_params.ConstraintWords) or None.  lora_tiles_view: the staged LoRA tile words or None."""
         mc = self.model_config
@@ -393,7 +393,8 @@ class LlamaModel:
         num_prefill_tokens = T - (B - P)
         sampling = None
         if words is not None:
-            sampling = SamplingState.from_staged(words, seq_lens if sampling_pos is None else sampling_pos, filtered, sampled)
+            sampling = SamplingState.from_staged(words, seq_lens if sampling_pos is None else sampling_pos, filtered, sampled,
+                                                 truncated)
             if sampling.penalized:
                 sampling = dataclasses.replace(
                     sampling, input_ids=ids, block_table=self.gpu_block_manager.block_table if block_table is None else block_table,
@@ -607,6 +608,7 @@ class LlamaModel:
             raise ValueError("forward_speculative does not apply penalties (their history is per position)")
         if has_ngram_controls(sampling_params_list):
             raise ValueError("forward_speculative does not apply no_repeat_ngram_size or DRY (their history is per position)")
+        truncated = has_truncation(sampling_params_list)
         con = constraint_words(token_masks_list, sampling_params_list, B, self.model_config.vocab_size, rows=rows)
         slots = self._lora_slots(lora_ids_list, B, False)
         if B == 0:
@@ -621,9 +623,10 @@ class LlamaModel:
         row_pos = [q + 1 for q in positions]             # sampling noise counter of row j: prefix + j + 1
         if samp is not None:
             # the words are per entry: every row of an entry gets its parameters and its seed
+            # (the min-p / typical-p / XTC words, when staged, follow the 5 * B sampling words: penalties are refused above)
             w = np.asarray(samp[0], dtype=np.int64)
             row_words = np.concatenate([w[:2 * B].reshape(B, 2)[rep].reshape(-1)] +
-                                       [w[(2 + s) * B:(3 + s) * B][rep] for s in range(3)]).tolist()
+                                       [w[(2 + s) * B:(3 + s) * B][rep] for s in range(3 + 4 * truncated)]).tolist()
         tiles = None if slots is None else lora_tiles(slots, rows)
         if tiles is not None:
             self.lora.ensure_rows(T)
@@ -638,7 +641,7 @@ class LlamaModel:
                                         max_decoding_len=0, decoding_lens=[], prefix=p_prefix,
                                         max_prefill_kv_len=max(seq_lengths), speculative=True,
                                         words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampling_pos=r_pos,
-                                        constraints=None if con is None else (views[1 if samp else 0], con),
+                                        truncated=truncated, constraints=None if con is None else (views[1 if samp else 0], con),
                                         lora_tiles_view=views[bool(samp) + bool(con)] if tiles else None)
         tokens = self._forward(ids, infer_state).tolist()
         out, keep = [], []
@@ -671,6 +674,7 @@ class LlamaModel:
         top_n = logprobs_top_n(sampling_params_list) if with_logprobs else None
         ngram = has_ngram_controls(sampling_params_list)
         penalized = ngram or has_penalties(sampling_params_list)
+        truncated = has_truncation(sampling_params_list)
         if ngram and ignore_kvcache:
             raise ValueError("no_repeat_ngram_size and DRY need the token history of the block table: not available with "
                              "ignore_kvcache")
@@ -713,7 +717,7 @@ class LlamaModel:
             self.lora.ensure_rows(num_tokens)
         if graph:
             return self._forward_decode_graph(flat_ids, seq_ids_list, list(decoding_seq_lens_list), max_decoding_len, samp,
-                                              top_n, penalized, sampled, con, slots, ngram)
+                                              top_n, penalized, sampled, con, slots, ngram, truncated)
         tiles = None if slots is None else lora_tiles(slots, prefill_lens + [1] * (batch_size - num_prefill_seqs))
 
         if not ignore_kvcache:
@@ -737,14 +741,14 @@ class LlamaModel:
             max_decoding_len=max_decoding_len, decoding_lens=list(decoding_seq_lens_list), prefix=p_prefix if chunked else None,
             max_prefill_kv_len=max(seq_lengths_list[:num_prefill_seqs]) if chunked else 0, ignore_kvcache=ignore_kvcache,
             words=views[0] if samp else None, filtered=bool(samp and samp[1]), sampled=sampled, top_n=top_n,
-            prompt_state=prompt_state, constraints=None if con is None else (views[1 if samp else 0], con),
+            truncated=truncated, prompt_state=prompt_state, constraints=None if con is None else (views[1 if samp else 0], con),
             lora_tiles_view=views[bool(samp) + bool(con)] if tiles else None)
         return self._forward(ids, infer_state)
 
     # ------------------------------------------------------------------ CUDA-graph decode path
     def _forward_decode_graph(self, flat_ids, seq_ids_list, lens_list, max_len, samp=None, top_n=None, penalized=False,
                               sampled=True, con: Optional[ConstraintWords] = None, slots: Optional[list] = None,
-                              ngram: bool = False):
+                              ngram: bool = False, truncated: bool = False):
         """Pure-decode step replayed from a CUDA graph.  The step's metadata is staged through the same pinned ring as an eager
         step's, into the graph's static device buffer, and its blocks are reserved on the manager's host mirror like an eager
         step's; the graph (keyed by batch size and the attention launch geometry) contains allocation-free work only: block
@@ -755,7 +759,8 @@ class LlamaModel:
         step with n-gram controls (`ngram`) the penalty kernel's n-gram launch, keyed by one more tag.  A
         constrained step (`con`: the graph-sized constraint region) has its own graph per bias capacity (the step's bias entries
         rounded up to a power of two), which also runs the constraint kernel.  An adapted step (`slots`, _lora_slots) has its own
-        graph, which also runs the LoRA kernels over a tile list padded to B tiles, so any mix of slots replays it."""
+        graph, which also runs the LoRA kernels over a tile list padded to B tiles, so any mix of slots replays it.  A step
+        with min-p / typical-p / XTC rows (`truncated`) has its own graph, which samples through the truncated entry."""
         from swiftllm_b200 import _lib
         self._check_shared_writes(seq_ids_list, [l - 1 for l in lens_list])
         B = len(flat_ids)
@@ -777,6 +782,8 @@ class LlamaModel:
             key += ("constrained", con.num_bias)
         if slots is not None:
             key += ("lora",)
+        if truncated:
+            key += ("truncated",)
         g = self._graphs.pop(key, None)
         if g is None:
             # bounded cache (least recently used graph dropped first); all graphs share ONE memory pool - they are replayed
@@ -786,7 +793,8 @@ class LlamaModel:
                 self._graphs.pop(next(iter(self._graphs)))
             g = self._capture_decode_graph(B, bucket, None if not samp else samp[1], top_n, penalized, sampled,
                                            None if con is None else con._replace(words=None),
-                                           **({} if slots is None else dict(lora=True)), **(dict(ngram=True) if ngram else {}))
+                                           **({} if slots is None else dict(lora=True)), **(dict(ngram=True) if ngram else {}),
+                                           **(dict(truncated=True) if truncated else {}))
         self._graphs[key] = g                    # (re)insert as most recently used
         # the blocks are counted on the host, and the eager step's errors raised, before anything is enqueued; the graph's
         # allocation kernel hands them out
@@ -804,16 +812,17 @@ class LlamaModel:
 
     def _capture_decode_graph(self, B: int, bucket_len: int, filtered: Optional[bool] = None, top_n: Optional[int] = None,
                               penalized: bool = False, sampled: bool = True, con: Optional[ConstraintWords] = None,
-                              lora: bool = False, ngram: bool = False):
+                              lora: bool = False, ngram: bool = False, truncated: bool = False):
         """filtered None: greedy graph; else a sampled graph whose meta starts with the 5 * B sampling words.  top_n: the graph
         also computes log-probabilities with this top-N.  penalized: the meta starts with 8 * B words (sampling and penalties),
         the graph penalises the logits and records the step's tokens in the token pages; `sampled` False takes the argmax.  ngram:
         the meta starts with 28 * B words (the n-gram controls follow the penalties; all zero, so off, during the warm-up).  con:
         the sizes of the graph's constraint region (words None), which follows the sampling words; the graph constrains the
-        logits first.  lora: B LoRA tiles follow (empty during the warm-up)."""
+        logits first.  lora: B LoRA tiles follow (empty during the warm-up).  truncated: 4 * B more sampling words (min-p,
+        typical-p, XTC) end the sampling words; the warm-up's temperatures are 0, so its rows are greedy."""
         ec = self.engine_config
         dev = self.device
-        nw = 0 if filtered is None else (28 if ngram else 8 if penalized else 5) * B
+        nw = 0 if filtered is None else (28 if ngram else 8 if penalized else 5) * B + (4 * B if truncated else 0)
         nc = 0 if con is None else ConstraintWords.size(*con[1:])
         nl = 3 * B if lora else 0
         meta = torch.zeros((nw + nc + nl + 3 * B,), dtype=torch.int32, device=dev)
@@ -831,6 +840,7 @@ class LlamaModel:
             st = self._infer_state(ids, seq_ids, lens, empty, empty, pos, last, max_prefill_len=0,
                                    max_decoding_len=bucket_len, decoding_lens=None,
                                    words=None if filtered is None else meta[:nw], filtered=filtered, sampled=sampled,
+                                   truncated=truncated,
                                    top_n=top_n, block_table=bm.block_table, token_cache=token_cache,
                                    constraints=None if con is None else (meta[nw:nw + nc], con),
                                    lora_tiles_view=meta[nw + nc:o] if lora else None)
